@@ -7,8 +7,11 @@
 
 Model/config: online SGD matrix factorisation, 10M users x 1M items, k=64, item vectors on the
 parameter server sharded over the N GPUs (psParallelism=N), user vectors on the owning worker
-(workerParallelism=N), synthetic uniform ratings, random-init factors.  One "step" = one
-micro-batch of ``--batch`` ratings per GPU pushed through the fused pull+SGD+push kernel; one
+(workerParallelism=N), synthetic uniform ratings, random-init factors.  One "step" = ``--batch``
+ratings per GPU pushed through the fused pull+SGD+push kernel, as ceil(batch / min(items, local users))
+conflict-free micro-batches (no user repeats within a step while the batch fits the local users, no item
+within a micro-batch: at N=1 every launch updates each row at most once, so a step's result does not
+depend on how the asynchronous kernel is scheduled); one
 "update" = one (user, item, rating) SGD update (pull item, update user, push item delta).
 
 Two measurements are printed on ONE JSON line by rank 0:
@@ -71,7 +74,49 @@ def parse():
                    help="do not bind the process to the NUMA node of its GPU (utils/numa.py)")
     p.add_argument("--kernel", default=None, choices=[None, "tma", "reg"],
                    help="fused MF kernel variant (default: reg = register-staged loads at full occupancy)")
-    return p.parse_args()
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write what they computed to DIR/<name>.npy (see dump_outputs)")
+    a = p.parse_args()
+    if a.dump_outputs and a.impl != "fps_b200":
+        p.error("--dump-outputs needs --impl fps_b200")
+    return a
+
+
+DUMP_SEED = 20251015
+DUMP_BYTES_PER_TABLE = 24 << 20      # ids + vectors of one table; two tables + stats stay below 64 MB
+
+
+def dump_outputs(directory, model, world, rank):
+    """The model state the timed steps leave behind, as a caller of ``DeviceOnlineMF.step`` sees it:
+
+    * ``stats.npy``         float64 [2]: (sum of squared errors, updates) of the last timed step;
+    * ``user_ids.npy``      float64 [m]: a fixed, seeded sample of rank 0's users (sorted; ids < 2^53 are exact);
+    * ``user_vectors.npy``  float32 [m, k]: their factor vectors;
+    * ``item_ids.npy``      float64 [m']: a fixed, seeded sample of all items (sorted);
+    * ``item_vectors.npy``  float32 [m', k]: their factor vectors, pulled from the parameter server.
+
+    At most 24 MB of ids + vectors per table (48 MB in all), so runs of two builds can be compared row for row.
+    At N=1 the micro-batches are conflict-free, so two runs with the same arguments write the same vectors
+    (``stats`` up to the order of its fp32 atomic sums)."""
+    import numpy as np
+    import torch
+
+    if rank != 0:
+        return
+    os.makedirs(directory, exist_ok=True)
+    k = model.k
+    m_max = max(1, DUMP_BYTES_PER_TABLE // (8 + 4 * k))      # float64 id + k float32 per row
+    g = torch.Generator().manual_seed(DUMP_SEED)
+    n_local = model.users.shape[0]
+    slots = torch.randperm(n_local, generator=g)[:m_max].sort().values
+    slots = slots[slots * world + rank < model.num_users]
+    uvec = model.users[slots.to(model.cuda_device), :k]
+    ids = torch.randperm(model.num_items, generator=g)[:m_max].sort().values
+    ivec = model.items.pull(ids.to(device=model.cuda_device, dtype=torch.int32))[:, :k]
+    out = {"stats": model.stats.double(), "user_ids": (slots * world + rank).double(), "user_vectors": uvec,
+           "item_ids": ids.double(), "item_vectors": ivec}
+    for name, t in out.items():
+        np.save(os.path.join(directory, name + ".npy"), t.cpu().numpy())
 
 
 class ClockSampler:
@@ -272,26 +317,46 @@ def main():
         from fps_b200.parallel.nccl_baseline import NcclOnlineMF as Model
     else:
         Model = DeviceOnlineMF
+    n_local_users = a.users // world  # every generated user id stays < users and owned by rank
+    n_sub = -(-a.batch // min(a.items, n_local_users))   # conflict-free micro-batches per step (see below)
     cache = {"auto": None, "on": True, "off": False}[a.item_cache]
     extra = {} if a.impl == "nccl" else {"item_blocking": {"auto": None, "on": True, "off": False}[a.item_blocking]}
     model = Model(a.users, a.items, a.factors, learning_rate=a.lr, pull_limit=a.pull_limit,
                   seed=1234, err_mode=ERR_SIGMOID if a.update_rule == "parity" else ERR_PLAIN,
                   kernel=a.kernel, item_cache=cache,
-                  sync_every=a.sync_every, **extra)
+                  # the replica policy counts step() calls: every row is still exchanged once per
+                  # --sync-every steps, one slice per micro-batch
+                  sync_every=a.sync_every * n_sub, **extra)
 
     # ---- synthetic ratings: users owned by this worker (user % W == rank), uniform items -------
+    # A step's ratings come as conflict-free micro-batches (distinct users in the step -- in each micro-batch
+    # when the batch exceeds the local users -- and distinct items in a micro-batch): the fused kernel then
+    # updates every row at most once per launch, and what a step computes is a function of its inputs alone,
+    # not of the order in which the asynchronous kernel's warps happen to run.
     g = torch.Generator().manual_seed(1000 + rank)
-    n_local_users = a.users // world  # every generated user id stays < users and owned by rank
-    host = []
+    sizes = [len(c) for c in torch.arange(a.batch).tensor_split(n_sub)]
+    host = []           # host[b] = the micro-batches of one step
     for _ in range(a.host_buffers):
-        u = torch.randint(0, n_local_users, (a.batch,), generator=g, dtype=torch.int32) * world + rank
-        i = torch.randint(0, a.items, (a.batch,), generator=g, dtype=torch.int32)
-        r = torch.rand(a.batch, generator=g, dtype=torch.float32).half().float()  # fp16-exact ratings
-        if a.format == "packed64" and a.impl == "fps_b200":
-            host.append((native.pack_ratings(u, i, r).pin_memory(),))
-        else:
-            host.append((u.pin_memory(), i.pin_memory(), r.pin_memory()))
-    devb = [tuple(t.to(dev) for t in b) for b in host]
+        step = []
+        if a.batch <= n_local_users:
+            step_users = torch.randperm(n_local_users, generator=g)[:a.batch].split(sizes)
+        for j, n in enumerate(sizes):
+            u = step_users[j] if a.batch <= n_local_users else torch.randperm(n_local_users, generator=g)[:n]
+            u = u.to(torch.int32) * world + rank
+            i = torch.randperm(a.items, generator=g)[:n].to(torch.int32)
+            r = torch.rand(n, generator=g, dtype=torch.float32).half().float()  # fp16-exact ratings
+            if a.format == "packed64" and a.impl == "fps_b200":
+                step.append((native.pack_ratings(u, i, r).pin_memory(),))
+            else:
+                step.append((u.pin_memory(), i.pin_memory(), r.pin_memory()))
+        host.append(step)
+    devb = [[tuple(t.to(dev) for t in b) for b in step] for step in host]
+
+    def run_step(m, s, reset_stats=False):
+        if reset_stats:
+            m.stats.zero_()    # the step's loss, as fit_stream reports it
+        for b in devb[s % len(devb)]:
+            m.step(*b)
 
     def barrier():
         torch.cuda.synchronize()
@@ -305,7 +370,7 @@ def main():
         sampler.start()
     windows = []
     for s in range(a.warmup):
-        model.step(*devb[s % len(devb)])
+        run_step(model, s, reset_stats=True)
     if hasattr(model, "flush"):
         model.flush()          # warm-up covers every kernel of the timed region, the end-of-run merge included
     barrier()
@@ -314,7 +379,7 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for s in range(a.steps):
-        model.step(*devb[(a.warmup + s) % len(devb)])
+        run_step(model, a.warmup + s, reset_stats=True)
     e_mid = torch.cuda.Event(enable_timing=True)
     e_mid.record()
     if hasattr(model, "flush"):
@@ -328,11 +393,14 @@ def main():
     barrier()
     ms_max = max_over_ranks(ms)
     model.check_finite()
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, model, world, rank)
+        barrier()          # the other ranks' shards stay as the timed steps left them until rank 0 has read them
 
     # ---- end to end through the public API -----------------------------------------------------
     def stream(n):
         for s in range(n):
-            yield host[s % len(host)]
+            yield from host[s % len(host)]
 
     for _ in model.fit_stream(stream(a.warmup)):
         pass
@@ -341,8 +409,11 @@ def main():
     t0 = time.perf_counter()
     e0.record()
     n_res = 0
-    last = (0.0, 0.0)
-    for last in model.fit_stream(stream(a.steps)):
+    last = [0.0, 0.0]        # (sum of squared errors, updates) of the last step's micro-batches
+    for sse, n in model.fit_stream(stream(a.steps)):
+        if n_res % n_sub == 0:
+            last = [0.0, 0.0]
+        last[0] += sse; last[1] += n
         n_res += 1
     e1.record()
     torch.cuda.synchronize()
@@ -350,8 +421,8 @@ def main():
     windows.append((w0, time.time()))
     e2e_ms = max(e0.elapsed_time(e1), wall_ms)
     e2e_ms_max = max_over_ranks(e2e_ms)
-    assert n_res == a.steps
-    h2d = sum(x.numel() * x.element_size() for x in host[0])
+    assert n_res == a.steps * n_sub
+    h2d = sum(x.numel() * x.element_size() for b in host[0] for x in b)
     barrier()
 
     # ---- the north-star path on the record: direct one-sided mode (every update pulls its item row from
@@ -362,12 +433,12 @@ def main():
                             seed=1234, err_mode=ERR_SIGMOID if a.update_rule == "parity" else ERR_PLAIN,
                             kernel=a.kernel, item_cache=False)
         for s in range(a.warmup):
-            dm.step(*devb[s % len(devb)])
+            run_step(dm, s)
         barrier()
         w0 = time.time()
         e0.record()
         for s in range(a.steps):
-            dm.step(*devb[(a.warmup + s) % len(devb)])
+            run_step(dm, a.warmup + s)
         e1.record()
         torch.cuda.synchronize()
         d_ms = max_over_ranks(e0.elapsed_time(e1))
@@ -388,12 +459,12 @@ def main():
         fm = DeviceOnlineMFf64(a.users, a.items, a.factors, learning_rate=a.lr, seed=1234,
                                err_mode=ERR_SIGMOID if a.update_rule == "parity" else ERR_PLAIN)
         for s in range(a.warmup):
-            fm.step(*devb[s % len(devb)])
+            run_step(fm, s)
         barrier()
         w0 = time.time()
         e0.record()
         for s in range(a.steps):
-            fm.step(*devb[(a.warmup + s) % len(devb)])
+            run_step(fm, a.warmup + s)
         e1.record()
         torch.cuda.synchronize()
         f_ms = max_over_ranks(e0.elapsed_time(e1))
@@ -430,13 +501,16 @@ def main():
             "config": {"model": "online SGD MF 10Mx1M k=64 (psOnlineMF)", "users": a.users,
                        "items": a.items, "factors": a.factors,
                        "global_batch": a.batch * world, "per_gpu_batch": a.batch,
+                       "micro_batches_per_step": n_sub,
                        "seq_len": None, "parallelism": f"workers{world}xps{world}",
                        "partition": "user%W on workers, item%G on PS shards",
                        "l2": "inputs larger than L2: 2.8 GB of factor tables accessed at random, "
-                             f"{len(host)} distinct {h2d >> 20} MiB rating batches cycled",
+                             f"{len(host)} distinct {h2d >> 20} MiB rating steps cycled",
                        "pull_limit": a.pull_limit or "hardware max rows in flight",
                        "item_cache": bool(getattr(model, "item_cache", False)),
                        "sync_every": a.sync_every,
+                       "sync_every_note": "in steps; the replica policy runs per micro-batch with "
+                                          f"sync_every={a.sync_every * n_sub} slices",
                        "item_blocking": (f"{model.block_buckets} buckets of {1 << model.block_shift} item rows, "
                                          "reordered inside the timed step (2 extra kernels)"
                                          if getattr(model, "item_blocking", False) else False),
@@ -460,7 +534,7 @@ def main():
             "value_fp64": fp64,
             "clocks": clocks,
             "e2e": {"value": e2e_value, "unit": "updates/s", "ms_per_step": e2e_ms_max / a.steps,
-                    "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 8,
+                    "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 8 * n_sub,
                     "last_step_mse": (last[0] / last[1]) if last[1] else None},
             "gpu_launches": launches,
         }

@@ -7,8 +7,8 @@ NCCL send/recv baseline.
 Every rank pulls (then pushes) `rows` vectors of `dim` floats that live on OTHER ranks' shards
 (ids owned by rank+1, rank+2, ... round robin), i.e. all traffic crosses NVLink.  Times are CUDA
 events on the launching stream, max over ranks; GB/s is per GPU per direction.  The NCCL arm moves the
-same bytes with batched isend/irecv between the same pairs.  Roofline: 770 GB/s measured peer copy
-per direction per GPU (900 nominal).
+same bytes with batched isend/irecv between the same pairs.  Roofline: 450 GB/s per direction per GPU,
+the NVLink 4 data-sheet rate of an H100 SXM (a ceiling, not a measured peer-copy rate).
 """
 import json
 import os
@@ -78,7 +78,7 @@ def main():
                "pull_ms": t_pull, "pull_GBs": nbytes / t_pull / 1e6,
                "push_ms": t_push, "push_GBs": nbytes / t_push / 1e6,
                "nccl_sendrecv_ms": t_nccl, "nccl_GBs": nbytes / t_nccl / 1e6 if world > 1 else None,
-               "pull_frac_of_770": nbytes / t_pull / 1e6 / 770.0}
+               "pull_frac_of_450": nbytes / t_pull / 1e6 / 450.0}
         if rank == 0:
             print(json.dumps(rec), flush=True)
         out.append(rec)

@@ -4,7 +4,7 @@ GPU 0 holds a replica (owner-major, 2 segments) and the master shard 0; master s
 HBM and is reached through peer access.  The exchange of destination 1 therefore moves every row over
 NVLink in both directions (bulk reads of v, REDG of d), exactly like one remote segment of an N-GPU job.
 
-    python benchmarks/exchange_peer_bench.py [--rows 500000] [--dim 64] [--ctas 32,64,148,296] [--stages 4]
+    python benchmarks/exchange_peer_bench.py [--rows 500000] [--dim 64] [--ctas 32,64,132,264] [--stages 4]
 
 Prints one JSON line: per CTA count the exchange time, GB/s per direction over the link and the local HBM
 bytes moved.  Under ncu add ``--once`` (one exchange per configuration, no timing loop).
@@ -23,7 +23,7 @@ def main():
     p = argparse.ArgumentParser()
     p.add_argument("--rows", type=int, default=500_000, help="rows per segment")
     p.add_argument("--dim", type=int, default=64)
-    p.add_argument("--ctas", default="16,32,64,148,296")
+    p.add_argument("--ctas", default="16,32,64,132,264")
     p.add_argument("--stages", type=int, default=4)
     p.add_argument("--iters", type=int, default=10)
     p.add_argument("--once", action="store_true")

@@ -1,7 +1,7 @@
 """CPU model of the replica (sender-side combining) mode's staleness: N workers train their own replica of the
 item table with mini-batched SGD and merge `replica - base` deltas every `sync_every` steps; held-out RMSE against
 ONE worker on the same stream and update budget.  Pure torch on the host -- a quick way to explore the
-quality side of the `sync_every` knob without a GPU (the measured GPU curves are in profiles/quality_curves_n8.json).
+quality side of the `sync_every` knob without a GPU.
 
     python benchmarks/replica_staleness_sim.py [--users 4096 --items 8192 --k 16 --lr 0.05 --updates 5242880]
 """

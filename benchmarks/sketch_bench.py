@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Streaming-sketch update throughput (K8-K10): (word, tweet) occurrences/s and one-sided reductions/s
-for Bloom (red.or.b32), tug-of-war (red.add.s32) and MinHash (red.min.u64) on one B200."""
+for Bloom (red.or.b32), tug-of-war (red.add.s32) and MinHash (red.min.u64) on one GPU."""
 import json
 import os
 import sys

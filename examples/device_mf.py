@@ -1,4 +1,4 @@
-"""Fused online SGD matrix factorisation on B200:  python examples/device_mf.py
+"""Fused online SGD matrix factorisation on an H100:  python examples/device_mf.py
    or  python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 examples/device_mf.py"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""Top-K serving on B200: user vectors on the parameter server, tcgen05 scoring against local items."""
+"""Top-K serving on an H100: user vectors on the parameter server, wgmma scoring against local items."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""fps_b200 -- a Blackwell (B200, sm_100a) native asynchronous parameter-server framework with
+"""fps_b200 -- a Hopper (H100, sm_90a) native asynchronous parameter-server framework with
 the capabilities of FlinkML/flink-parameter-server.
 
 Public surface (reference names kept):
@@ -9,7 +9,7 @@ Public surface (reference names kept):
 * ``addPullLimiter``, ``addBlockingPullLimiter``, ``WorkerLogicWithFuture``
 * server stores in :mod:`fps_b200.server`, wire protocol / batching in :mod:`fps_b200.protocol`
 * algorithms in :mod:`fps_b200.models` (matrix factorisation, passive-aggressive, sketches, ...)
-* device tier: :mod:`fps_b200.store` (sharded HBM tables), :mod:`fps_b200.ops` (sm_100a kernels),
+* device tier: :mod:`fps_b200.store` (sharded HBM tables), :mod:`fps_b200.ops` (sm_90a kernels),
   :mod:`fps_b200.parallel` (NVLink symmetric-heap fabric, partitioners, NCCL baseline)
 """
 from .api import (BatchedParameterServerClient, BatchedWorkerLogic, Either, Left,

@@ -13,7 +13,7 @@ reference                          here
 ``Either`` outputs                 :class:`Left` (worker output) / :class:`Right` (PS output)
 =================================  ==========================================================
 
-On top of the per-record callbacks the B200 design adds *batched* callbacks
+On top of the per-record callbacks the device design adds *batched* callbacks
 (:class:`BatchedWorkerLogic`): a worker receives a micro-batch of records and pulls / pushes whole
 id tensors, which the device backend executes as fused gather / red.add kernels over NVLink peer
 memory.  Per-record logics run unchanged on every backend through the scalar adapter.
@@ -139,7 +139,7 @@ class WorkerLogic(LooseWorkerLogic[T, Id, P, P, WOut]):
 
 
 class BatchedWorkerLogic(WorkerLogic):
-    """Micro-batch worker callbacks (B200 extension; see module docstring).
+    """Micro-batch worker callbacks (device-tier extension; see module docstring).
 
     ``onRecvBatch`` gets a batch object (any structure of tensors) and a
     :class:`BatchedParameterServerClient`; ``onPullRecvBatch`` gets the id tensor of a pull and

@@ -1,4 +1,4 @@
-"""Device (B200) implementation of online / offline SGD matrix factorisation.
+"""Device (H100) implementation of online / offline SGD matrix factorisation.
 
 Capability parity with ``PSOnlineMatrixFactorization.psOnlineMF`` and
 ``PSOfflineMatrixFactorization.psOfflineMF`` (reference:
@@ -9,7 +9,7 @@ M/matrix/factorization/workers/PSOnlineMatrixFactorizationWorker.scala:22-90):
 * item vectors live on the parameter server, sharded ``item % psParallelism``,
 * every rating triggers pull(item) -> SGD delta -> local user update -> push(item delta).
 
-B200-first mechanism: one process per GPU is both worker ``rank`` and PS shard ``rank``; the whole
+Device mechanism: one process per GPU is both worker ``rank`` and PS shard ``rank``; the whole
 worker step for a micro-batch is ONE kernel (``fps_mf_sgd_fused``) that pulls item rows with
 16-byte loads from the owner's HBM over NVSwitch, computes the update and pushes the delta back
 with ``red.global.add.v4.f32`` -- no messages, no NCCL, no separate elementwise kernel.

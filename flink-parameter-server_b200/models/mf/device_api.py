@@ -158,7 +158,7 @@ def ps_topk_generator_device(src, model, K: int = 100, workerK: int = 75, userMe
                              batch_size: int = 4096, group=None, sort_by_length: bool = True):
     """Top-K serving over a pre-trained model on the device tier (capability of ``psTopKGenerator``,
     PSTopKGenerator.scala:47-107): the user vectors of ``model`` are loaded into a sharded PS table, the
-    item vectors stay with this worker, every query is scored on the tcgen05 kernel (length-sorted item
+    item vectors stay with this worker, every query is scored on the wgmma kernel (length-sorted item
     table = the LEMP LENGTH bound) and the per-worker lists are merged.  ``model`` has the reference's
     orientation: ``Left((itemId, (len, vec)))`` / ``Right((userId, (len, vec)))``.  In a multi-rank job
     every rank passes its own part of the model and the *same* query stream.  Unknown users get an empty
@@ -245,7 +245,7 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
     vectors on the workers** (rank ``item % N`` owns the item).  Every rank is handed the same rating
     stream (the reference broadcasts each rating to all workers, ``:84-101``).  Per micro-batch:
 
-    1. every rank scores the batch's users -- pulled from the PS by the tcgen05 kernel's A-gather --
+    1. every rank scores the batch's users -- pulled from the PS by the wgmma kernel's A-gather --
        against ITS item partition (``fps_topk_mma``) and keeps ``workerK`` candidates;
     2. the partial lists travel to the merge rank as one-sided stores (:class:`P2PGather`) and are
        merged by ``fps_row_topk`` (``CollectTopKFromEachWorker.scala:41-56``; seen-item filter on the host);

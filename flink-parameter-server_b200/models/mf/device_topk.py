@@ -1,5 +1,5 @@
 """Device top-K recommendation (K6 / K12): pull query vectors from the PS, score them against the
-worker-local item table on the tcgen05 tensor cores, keep an exact top-K.
+worker-local item table on the Hopper tensor cores (wgmma), keep an exact top-K.
 
 Capability of ``psTopKGenerator`` / the generator half of ``psOnlineLearnerAndGenerator``
 (PSTopKGenerator.scala:47-107, PSTopKGeneratorWorker.scala:35-114): user vectors live on the PS,
@@ -50,9 +50,8 @@ class DeviceTopK:
         self.max_batch_bytes = max_batch_bytes
         # theta is computed from the first `pass1_fraction` of the tiles only: the K-th largest tile maximum
         # of ANY subset of tiles is still a valid lower bound (K distinct items reach it), just a weaker
-        # one -- pass 1 shrinks to that fraction, pass 2 keeps a few more candidates.  Measured (2048
-        # queries x 1M items, K=100, profiles/topk_bench_pass1.json): 0.94 ms vs 1.04 ms with identical
-        # results, so 1/8 is the default for tables of >= 512 tiles (0 / None: scan every tile in pass 1).
+        # one -- pass 1 shrinks to that fraction, pass 2 keeps a few more candidates (identical results).
+        # 1/8 is the default for tables of >= 512 tiles (0 / None: scan every tile in pass 1).
         if pass1_fraction is None:
             pass1_fraction = 0.125 if self.n_tiles >= 512 else 0.0
         self.pass1_fraction = pass1_fraction

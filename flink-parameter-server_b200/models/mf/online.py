@@ -8,7 +8,7 @@ output((user, vec)) -> push(item, delta).
 
 ``backend="local"`` runs the per-record logic on the host tier (exact reference semantics incl.
 per-user negative-sampling memory); ``backend="device"`` runs the same algorithm as fused
-micro-batch kernels on B200 (:class:`fps_b200.models.mf.device.DeviceOnlineMF`).
+micro-batch kernels on the GPU (:class:`fps_b200.models.mf.device.DeviceOnlineMF`).
 
 The reference passes ``(negativeSampleRate, userMemory)`` into a ctor declared
 ``(userMemory, negativeSampleRate)`` (SURVEY §7.4); here the arguments mean what they say.
@@ -123,7 +123,7 @@ def psOnlineMF(src, numFactors: int = 10, rangeMin: float = -0.01, rangeMax: flo
                plain_residual: bool = False, backend: str = "local", **device_kw):
     """Returns the stream of ``Left((userId, userVector))`` / ``Right((itemId, itemVector))``.
     ``backend="local"``: arbitrary-logic Python engine; ``"native"``: the same protocol on the C++ host
-    engine (threads + SPSC rings, ``ops/csrc/fps_host.cpp``); ``"device"``: fused B200 kernels."""
+    engine (threads + SPSC rings, ``ops/csrc/fps_host.cpp``); ``"device"``: fused GPU kernels."""
     hostPullLimit = 1600 if pullLimit is None else pullLimit   # reference default (JVM queue bound)
     if backend == "native":
         from .native_api import ps_mf_native

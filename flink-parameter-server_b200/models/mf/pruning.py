@@ -6,7 +6,7 @@ Predicates (LEMPPruningFunctions.scala:20-89) take ``(itemId, (length, vector))`
 the item *may* still beat the current threshold (True = keep as candidate).
 
 The device tier keeps the string-configurable strategies but realises pruning at tile
-granularity inside the tcgen05 scoring kernel (length bound per 128-item tile of the
+granularity inside the wgmma scoring kernel (length bound per 128-item tile of the
 length-sorted item table; ops/csrc/fps_topk_mma.cu); every pruned result is validated against
 brute force in the tests because the reference's bounds are themselves untested (SURVEY §7.4).
 """

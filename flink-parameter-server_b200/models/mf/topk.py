@@ -11,7 +11,7 @@
 
 Every rating is broadcast to all workers (``RichRating(base, targetWorker, ratingId)``); worker w
 scans its local items bucket by bucket in descending length order with LEMP pruning.
-Device tier: models/mf/device_topk.py (pull user vectors + tcgen05 GEMM + top-K select).
+Device tier: models/mf/device_topk.py (pull user vectors + wgmma GEMM + top-K select).
 """
 from __future__ import annotations
 
@@ -178,7 +178,7 @@ def psTopKGenerator(src, model, numFactors: int = 10, rangeMin: float = -0.01, r
                     backend: str = "local", **device_kw):
     """``model``: stream of ``Left((itemId, (len, vec)))`` (to workers) / ``Right((userId, (len, vec)))``
     (to the PS) -- note the reference's Either orientation is kept.  Returns
-    ``[(itemId, timestamp, [(score, itemId)])]`` per rating.  ``backend="device"``: tcgen05 scoring
+    ``[(itemId, timestamp, [(score, itemId)])]`` per rating.  ``backend="device"``: wgmma scoring
     against a length-sorted item table (``models/mf/device_api.py::ps_topk_generator_device``)."""
     if backend == "device":
         from .device_api import ps_topk_generator_device

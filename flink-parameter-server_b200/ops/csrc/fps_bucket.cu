@@ -3,10 +3,10 @@
 //
 // Why: one update touches a user row and an item row.  The user side is compulsory HBM traffic (10M
 // users, every row read once and written once), but the item table (1M x 256 B = 256 MB) is hit ~4x
-// per 4M-rating micro-batch and is only twice the size of the 126 MB L2: processed in arrival order
-// about half of the item reads miss and most REDG-dirtied lines are written back before their next use
-// (ncu: 458 B read + 465 B written per update).  Dealing the ratings into buckets of <= 16 MB of item
-// rows turns the item side into one streaming pass per bucket (~61 B + 61 B per update).  Asynchronous
+// per 4M-rating micro-batch and is five times the size of the 50 MB L2 of an H100: processed in arrival
+// order most item reads miss and most REDG-dirtied lines are written back before their next use.
+// Dealing the ratings into buckets of <= 16 MB of item rows (a third of the L2) turns the item side into
+// one streaming pass per bucket.  Asynchronous
 // SGD has no ordering contract inside a micro-batch (the reference's workers interleave arbitrarily),
 // so the reordering is semantically free.
 //

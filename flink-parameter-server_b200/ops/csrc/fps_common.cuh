@@ -1,4 +1,4 @@
-// Shared device-side definitions for the fps_b200 kernel library (sm_100a only).
+// Shared device-side definitions for the fps_b200 kernel library (sm_90a).
 //
 // A "ShardTable" is the device view of one parameter-server table: G shards (one per
 // GPU / PS instance), each a dense row-major [rows_per_shard, stride] fp32 block living

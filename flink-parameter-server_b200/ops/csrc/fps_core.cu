@@ -1,4 +1,4 @@
-// Core parameter-server kernels for sm_100a: lazy-init materialisation (K4), fused
+// Core parameter-server kernels for sm_90a: lazy-init materialisation (K4), fused
 // pull + SGD + push for matrix factorisation (K1+K3+K2), standalone pull gather (K1),
 // push accumulate (K2) and pull-fused-with-dot scoring.  All "communication" is done by
 // the kernels themselves through peer-mapped shard pointers (NVLink/NVSwitch one-sided
@@ -48,7 +48,7 @@ extern "C" int fps_init_rows(float* rows, long long n_rows, int dim, int stride,
   long long total = n_rows * (stride / 4);
   int threads = 256;
   long long blocks = (total + threads - 1) / threads;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;  // 32 CTAs per H100 SM, grid-stride beyond
   fps_init_rows_kernel<<<(int)blocks, threads, 0, stream>>>(rows, n_rows, dim, stride, shard,
                                                             num_shards, mode, div, seed, lo, hi);
   return (int)cudaGetLastError();

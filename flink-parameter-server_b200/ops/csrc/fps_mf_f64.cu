@@ -167,7 +167,7 @@ extern "C" int fps_init_rows_f64(double* rows, long long n_rows, int dim, int st
   if (n_rows <= 0) return 0;
   long long total = n_rows * (stride_d / 2);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;  // 32 CTAs per H100 SM, grid-stride beyond
   fps_init_rows_f64_kernel<<<(int)blocks, 256, 0, stream>>>(rows, n_rows, dim, stride_d, shard, num_shards, mode,
                                                             div, seed, lo, hi);
   return (int)cudaGetLastError();

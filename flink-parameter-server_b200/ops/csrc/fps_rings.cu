@@ -1,7 +1,7 @@
 // Message tier on the device: peer-memory request / response rings, a persistent server kernel and
 // a device-side credit counter (pull limiter).
 //
-// This is the B200 replacement of the reference's iteration feedback edge (FPS:447-480) for the
+// This is the GPU replacement of the reference's iteration feedback edge (FPS:447-480) for the
 // stores that need *logic* on the server (per-key locks, non-commutative paramUpdate): the fused
 // kernels of fps_core.cu cover additive updates with zero messages, everything else goes through
 // these rings.

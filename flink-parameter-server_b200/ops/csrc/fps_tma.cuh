@@ -1,4 +1,4 @@
-// mbarrier + TMA 1-D bulk-copy helpers shared by the pipelined kernels (sm_100a).
+// mbarrier + TMA 1-D bulk-copy helpers shared by the pipelined kernels (sm_90a).
 //   cp.async.bulk            -> SASS UBLKCP   (global, local HBM or NVLink peer  ->  shared)
 //   cp.reduce.async.bulk.add -> SASS UBLKRED  (shared -> global reduction executed by the owner's L2)
 #pragma once

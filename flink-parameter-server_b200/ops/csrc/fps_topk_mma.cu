@@ -1,17 +1,16 @@
-// K6: pull (query vectors from the PS shards over NVLink) fused with a tcgen05 GEMM against the
-// worker-local item table and a top-K candidate-filter epilogue.  sm_100a only.
+// K6: pull (query vectors from the PS shards over NVLink) fused with a wgmma GEMM against the
+// worker-local item table and a top-K candidate-filter epilogue.  sm_90a (Hopper).
 //
-//   scores[q, i] = <query[q, :], item[i, :]>        (TF32 tensor-core MMA, FP32 accumulate in TMEM)
+//   scores[q, i] = <query[q, :], item[i, :]>        (TF32 tensor-core MMA, FP32 accumulate in registers)
 //
-//   A operand (queries, 128 rows/CTA): gathered ONCE per CTA from the owning PS shards with 16-byte
-//       peer loads and written into shared memory in the canonical K-major SWIZZLE_128B layout
+//   A operand (queries, 128 rows per query block): gathered ONCE per CTA from the owning PS shards with
+//       16-byte peer loads and written into shared memory in the canonical K-major SWIZZLE_128B layout
 //       (manual XOR swizzle), then published to the async proxy with fence.proxy.async.
-//   B operand (items): streamed by TMA (cp.async.bulk.tensor.2d, SASS UTMALDG) through a 4-stage
-//       mbarrier ring, hardware-swizzled by the tensor map.
-//   MMA: one elected thread issues tcgen05.mma.cta_group::1.kind::tf32 (SASS UTCHMMA-family), M=128,
-//       N=128, K=8 per instruction; two 128-column accumulators in TMEM are double buffered so the
-//       epilogue of tile t overlaps the MMAs of tile t+1 (tcgen05.commit -> mbarrier).
-//   Epilogue (4 warps, one TMEM lane = one query row per thread, tcgen05.ld 32x32b):
+//   B operand (items): streamed by TMA (cp.async.bulk.tensor.2d, SASS UTMALDG) through a 2..4-stage
+//       mbarrier ring by one producer warp, hardware-swizzled by the tensor map.
+//   MMA: 2 * MB consumer warpgroups of 64 query rows issue wgmma.m64n128k8 TF32 from smem descriptors
+//       into register accumulators; a retired stage is released before the epilogue (TMA overlaps it).
+//   Epilogue (wgmma fragment: each thread holds 32 columns of 2 rows, 4 lanes share a row):
 //       mode 0: write raw scores                    (small problems / validation)
 //       mode 1: per-(row, tile) maximum             (pass 1: gives an exact top-K lower bound theta)
 //       mode 2: append (score, item) >= theta[row]  (pass 2: exact candidate set, usually << N)
@@ -23,11 +22,10 @@
 #include <cuda.h>
 #include "fps_common.cuh"
 
-#define TK_M 128          // query rows per CTA (UMMA M)
-#define TK_N 128          // items per tile (UMMA N)
+#define TK_M 128          // query rows per query block (two wgmma M=64 warpgroups)
+#define TK_N 128          // items per tile (wgmma N)
 #define TK_KB_FLOATS 32   // floats per 128-byte swizzle atom row
 #define TK_MAX_STAGES 4
-#define TK_THREADS 256
 #define TK_MAX_KB 4       // dim <= 128 (A block + >= 2 B stages must fit in 227 KB of smem)
 
 struct TopkArgs {
@@ -92,63 +90,53 @@ __device__ __forceinline__ void tk_tma_load_2d(void* dst, const CUtensorMap* map
       "l"(map), "r"(tk_smem(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (SmemDescriptor, version 1 = sm_100)
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA descriptor): start address,
+// leading byte offset (unused by swizzled K-major layouts), stride byte offset = 8 rows * 128 B,
+// layout type 1 = SWIZZLE_128B.  Every operand block starts 1024-byte aligned (base offset 0).
 __device__ __forceinline__ uint64_t tk_desc(uint32_t smem_addr) {
   uint64_t d = (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)(1024u >> 4) << 32;  // stride byte offset: 8 rows * 128 B
-  d |= (uint64_t)1 << 46;             // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;             // SWIZZLE_128B
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(1024u >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-__device__ __forceinline__ void tk_mma_tf32(uint32_t tmem_c, uint64_t da, uint64_t db, uint32_t idesc,
-                                            uint32_t accumulate) {
+// d[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T, both K-major in shared memory; scale_d == 0 overwrites d.
+__device__ __forceinline__ void tk_wgmma_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_c),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tk_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   tk_smem(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tk_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
 
-// MB = number of 128-row query blocks per CTA.  With MB = 2 every item tile fetched by TMA feeds two
-// UMMA_M=128 accumulators (256 query rows), which halves the L2 -> SM item traffic per FLOP; the CTA
-// then has 8 epilogue warps (warps 4..11) and uses all 512 TMEM columns (2 blocks x 2 buffers x 128).
+// MB = number of 128-row query blocks per CTA.  With MB = 2 every item tile fetched by TMA feeds four
+// 64-row warpgroups (256 query rows), which halves the L2 -> SM item traffic per FLOP.
+// Warps 0 .. 8*MB-1 are the consumer warpgroups, warp 8*MB is the TMA producer.
 template <typename IdT, int MODE, int MB>
-__global__ void __launch_bounds__(128 + 128 * MB, 1)
+__global__ void __launch_bounds__(256 * MB + 32, 1)
     fps_topk_mma_kernel(const __grid_constant__ CUtensorMap item_map,
                         const __grid_constant__ TopkArgs a) {
   extern __shared__ __align__(1024) unsigned char tk_smem_raw[];
   const int KB = (a.stride + TK_KB_FLOATS - 1) / TK_KB_FLOATS;  // 128-byte K blocks
   const uint32_t kb_bytes = TK_M * 128;                         // one K block of a 128-row tile
-  unsigned char* sA = tk_smem_raw;                              // [MB][KB][128 rows][128 B]
+  // SWIZZLE_128B operands start 1024-byte aligned (the launcher adds 1 KB of slack for this)
+  unsigned char* sA = tk_smem_raw + ((1024u - (tk_smem(tk_smem_raw) & 1023u)) & 1023u);  // [MB][KB][128][128 B]
   unsigned char* sB = sA + (size_t)MB * KB * kb_bytes;          // [STAGES][KB][128 rows][128 B]
   const int NS = a.n_stages;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sB + (size_t)NS * KB * kb_bytes);
-  uint64_t* full = bars;                  // [STAGES] TMA -> MMA
-  uint64_t* empty = bars + TK_MAX_STAGES;     // [STAGES] MMA -> TMA
-  uint64_t* tfull = bars + 2 * TK_MAX_STAGES;   // [2] MMA -> epilogue
-  uint64_t* tempty = tfull + 2;             // [2] epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* full = bars;                      // [STAGES] TMA -> MMA
+  uint64_t* empty = bars + TK_MAX_STAGES;     // [STAGES] MMA -> TMA (one arrive per consumer warp)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -165,22 +153,12 @@ __global__ void __launch_bounds__(128 + 128 * MB, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < NS; ++s) {
       tk_mbar_init(&full[s], 1);
-      tk_mbar_init(&empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      tk_mbar_init(&tfull[s], 1);
-      tk_mbar_init(&tempty[s], 4 * MB);  // one arrive per epilogue warp
+      tk_mbar_init(&empty[s], 8 * MB);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {  // TMEM: 2 accumulators x 128 fp32 columns
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     tk_smem(tmem_slot)),
-                 "r"(256 * MB));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
 
-  // ---- A operand: pull the 128 query rows (peer loads) into swizzled smem ------------------
+  // ---- A operand: pull the query rows (peer loads) into swizzled smem ------------------------
   {
     const IdT* qids = reinterpret_cast<const IdT*>(a.q_ids);
     const int nvec = a.stride >> 2;
@@ -202,12 +180,9 @@ __global__ void __launch_bounds__(128 + 128 * MB, 1)
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic writes -> async proxy
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8 * MB) {
     // =============================== TMA producer (items) ===============================
     if (lane == 0) {
       for (int i = 0; i < my_tiles; ++i) {
@@ -221,130 +196,132 @@ __global__ void __launch_bounds__(128 + 128 * MB, 1)
                          &full[s]);
       }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    // instruction descriptor: D=F32, A=B=TF32, K-major x K-major, N=128, M=128
-    const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TK_N >> 3) << 17) |
-                           ((uint32_t)(TK_M >> 4) << 24);
-    if (lane == 0) {
-      for (int i = 0; i < my_tiles; ++i) {
-        const int s = i % NS;
-        const uint32_t ph = (uint32_t)((i / NS) & 1);
-        const int acc = i & 1;
-        const uint32_t aph = (uint32_t)((i >> 1) & 1);
-        tk_mbar_wait(&tempty[acc], aph ^ 1u);  // epilogue drained this accumulator
-        tk_mbar_wait(&full[s], ph);            // TMA landed the item tile
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-        for (int mb = 0; mb < MB; ++mb) {
-          const uint32_t d_tmem = tmem_base + (uint32_t)(acc * MB + mb) * TK_N;
-          for (int kb = 0; kb < KB; ++kb) {
-            const uint32_t a_addr = tk_smem(sA + ((size_t)mb * KB + kb) * kb_bytes);
-            const uint32_t b_addr = tk_smem(sB + ((size_t)s * KB + kb) * kb_bytes);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {  // UMMA_K = 8 tf32 = 32 bytes inside the 128-byte atom
-              tk_mma_tf32(d_tmem, tk_desc(a_addr + k * 32), tk_desc(b_addr + k * 32), idesc,
-                          (kb | k) != 0 ? 1u : 0u);
-            }
-          }
-        }
-        tk_commit(&empty[s]);     // smem stage reusable once these MMAs retire
-        tk_commit(&tfull[acc]);   // accumulator ready for the epilogue
-      }
-    }
-  } else if (warp >= 4) {
-    // =============================== epilogue ===============================
-    const int ew = warp & 3;                    // TMEM lane quadrant this warp may access
-    const int emb = (warp - 4) >> 2;            // which 128-row query block this warp drains
-    const int r = emb * TK_M + ew * 32 + lane;  // row inside the CTA's query rows
-    const int row = row0 + r;
-    const bool row_ok = row < a.n_queries;
-    const float th = (MODE == 2 && row_ok) ? a.theta[row] : 0.f;
-    int n_cand = 0;
-    float* seg_s = nullptr;
-    int* seg_i = nullptr;
-    if (MODE == 2 && row_ok) {
-      seg_s = a.cand_score + (size_t)row * a.cand_cap + (size_t)split * a.seg_cap;
-      seg_i = a.cand_item + (size_t)row * a.cand_cap + (size_t)split * a.seg_cap;
-    }
-    for (int i = 0; i < my_tiles; ++i) {
-      const int acc = i & 1;
-      const uint32_t aph = (uint32_t)((i >> 1) & 1);
-      const int tile = first_tile + i * a.n_splits;
-      const int item0 = tile * TK_N;
-      const bool full_tile = item0 + TK_N <= a.n_items;   // no per-element bound check needed
-      tk_mbar_wait(&tfull[acc], aph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      float tmax = -3.0e38f;
-#pragma unroll 1
-      for (int c0 = 0; c0 < TK_N; c0 += 32) {
-        uint32_t v[32];
-        __syncwarp();  // tcgen05.ld is .sync.aligned: the whole warp must be converged here
-        tk_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)((acc * MB + emb) * TK_N + c0), v);
-        if (row_ok) {
-        if (MODE == 1) {
-          if (full_tile) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) tmax = fmaxf(tmax, __uint_as_float(v[j]));
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (item0 + c0 + j < a.n_items) tmax = fmaxf(tmax, __uint_as_float(v[j]));
-          }
-        } else if (MODE == 2) {
-          // candidates are rare: first a branch-free "any >= theta" test over the 32 columns.  The
-          // thread owns (row, split) for the whole kernel, so candidates go to a private segment of the
-          // row's buffer with a register cursor: no atomics, no memory round trip in the epilogue
-          // (a returning atomic per candidate / per chunk made pass 2 latency bound).
-          // The test is hierarchical (4 groups of 8 columns): when one lane of the warp has a candidate
-          // the whole warp walks the predicated append loop, so the loop is kept to the 8 columns of
-          // the group that actually reached theta instead of all 32.
-          float gmax[4];
-#pragma unroll
-          for (int gi = 0; gi < 4; ++gi) {
-            float m = __uint_as_float(v[8 * gi]);
-#pragma unroll
-            for (int j = 1; j < 8; ++j) m = fmaxf(m, __uint_as_float(v[8 * gi + j]));
-            gmax[gi] = m;
-          }
-          if (fmaxf(fmaxf(gmax[0], gmax[1]), fmaxf(gmax[2], gmax[3])) >= th) {
-#pragma unroll
-            for (int gi = 0; gi < 4; ++gi) {
-              if (gmax[gi] >= th) {
-#pragma unroll
-                for (int j = 8 * gi; j < 8 * gi + 8; ++j) {
-                  const int item = item0 + c0 + j;
-                  const float sc = __uint_as_float(v[j]);
-                  if (sc >= th && (full_tile || item < a.n_items)) {
-                    if (n_cand < a.seg_cap) {
-                      seg_s[n_cand] = sc;
-                      seg_i[n_cand] = item;
-                    }
-                    ++n_cand;
-                  }
-                }
-              }
-            }
-          }
-        } else {
-          float* out = a.out_scores + (size_t)row * a.out_ld + item0 + c0;
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (full_tile || item0 + c0 + j < a.n_items) out[j] = __uint_as_float(v[j]);
-        }
-        }  // row_ok
-      }
-      if (MODE == 1 && row_ok) a.tile_max[(size_t)row * a.n_tiles + tile] = tmax;
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) tk_mbar_arrive(&tempty[acc]);
-    }
-    if (MODE == 2 && row_ok) a.cand_count[(size_t)row * a.n_splits + split] = n_cand;
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256 * MB));
+
+  // =============================== MMA + epilogue (consumer warpgroups) ===============================
+  const int wg = warp >> 2;                 // consumer warpgroup: 64 query rows
+  const int emb = wg >> 1;                  // which 128-row query block (A operand block)
+  const int half = wg & 1;                  // which 64-row half of it
+  // fragment of m64nNk8 with f32 accumulators: d[i] is (row rq + 8 * ((i >> 1) & 1),
+  // column 8 * (i >> 2) + 2 * (lane & 3) + (i & 1)) of the warpgroup's 64 x 128 tile
+  const int rq = emb * TK_M + half * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int rowA = row0 + rq, rowB = rowA + 8;
+  const bool okA = rowA < a.n_queries, okB = rowB < a.n_queries;
+  const int col0 = 2 * (lane & 3);
+  const float thA = (MODE == 2 && okA) ? a.theta[rowA] : 0.f;
+  const float thB = (MODE == 2 && okB) ? a.theta[rowB] : 0.f;
+  int candA = 0, candB = 0;                 // per-(row, split) cursor, identical in the row's 4 lanes
+  const uint32_t a_base = tk_smem(sA + (size_t)emb * KB * kb_bytes + (size_t)half * 64 * 128);
+  float d[64];
+#pragma unroll
+  for (int j = 0; j < 64; ++j) d[j] = 0.f;
+
+  for (int i = 0; i < my_tiles; ++i) {
+    const int s = i % NS;
+    const uint32_t ph = (uint32_t)((i / NS) & 1);
+    const int tile = first_tile + i * a.n_splits;
+    const int item0 = tile * TK_N;
+    const bool full_tile = item0 + TK_N <= a.n_items;   // no per-element bound check needed
+    tk_mbar_wait(&full[s], ph);                         // TMA landed the item tile
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+    const uint32_t b_base = tk_smem(sB + (size_t)s * KB * kb_bytes);
+#pragma unroll 1
+    for (int kb = 0; kb < KB; ++kb) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k)  // wgmma K = 8 tf32 = 32 bytes inside the 128-byte atom
+        tk_wgmma_tf32(d, tk_desc(a_base + kb * kb_bytes + k * 32), tk_desc(b_base + kb * kb_bytes + k * 32),
+                      (kb | k) != 0 ? 1u : 0u);
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    __syncwarp();
+    if (lane == 0) tk_mbar_arrive(&empty[s]);           // smem stage reusable: the MMAs have read it
+
+    if (MODE == 1) {
+      float mA = -3.0e38f, mB = -3.0e38f;
+#pragma unroll
+      for (int j = 0; j < 64; ++j) {
+        const int item = item0 + 8 * (j >> 2) + col0 + (j & 1);
+        if (full_tile || item < a.n_items) {
+          if ((j >> 1) & 1) mB = fmaxf(mB, d[j]); else mA = fmaxf(mA, d[j]);
+        }
+      }
+      mA = fmaxf(mA, __shfl_xor_sync(0xffffffffu, mA, 1));
+      mA = fmaxf(mA, __shfl_xor_sync(0xffffffffu, mA, 2));
+      mB = fmaxf(mB, __shfl_xor_sync(0xffffffffu, mB, 1));
+      mB = fmaxf(mB, __shfl_xor_sync(0xffffffffu, mB, 2));
+      if ((lane & 3) == 0) {
+        if (okA) a.tile_max[(size_t)rowA * a.n_tiles + tile] = mA;
+        if (okB) a.tile_max[(size_t)rowB * a.n_tiles + tile] = mB;
+      }
+    } else if (MODE == 2) {
+      // candidates are rare: first a branch-free "any >= theta" test over the thread's 64 values; the
+      // warp walks the append path only when one of its rows reached theta.  Each (row, split) owns a
+      // private segment of the row's buffer and a register cursor shared by the row's 4 lanes: no
+      // atomics (a returning atomic per candidate made pass 2 latency bound).
+      float mA = -3.0e38f, mB = -3.0e38f;
+#pragma unroll
+      for (int j = 0; j < 64; ++j) {
+        if ((j >> 1) & 1) mB = fmaxf(mB, d[j]); else mA = fmaxf(mA, d[j]);
+      }
+      const bool hit = (okA && mA >= thA) || (okB && mB >= thB);
+      if (__any_sync(0xffffffffu, hit)) {
+        int nA = 0, nB = 0;
+#pragma unroll
+        for (int j = 0; j < 64; ++j) {
+          const int item = item0 + 8 * (j >> 2) + col0 + (j & 1);
+          const bool in = full_tile || item < a.n_items;
+          if ((j >> 1) & 1) nB += (okB && in && d[j] >= thB) ? 1 : 0;
+          else nA += (okA && in && d[j] >= thA) ? 1 : 0;
+        }
+        // exclusive prefix of the counts over the row's 4 lanes (lane & 3 = 0..3)
+        int pA = nA, pB = nB;
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1) {
+          const int tA = __shfl_up_sync(0xffffffffu, pA, o, 4);
+          const int tB = __shfl_up_sync(0xffffffffu, pB, o, 4);
+          if ((lane & 3) >= o) { pA += tA; pB += tB; }
+        }
+        const int totA = __shfl_sync(0xffffffffu, pA, 3, 4);
+        const int totB = __shfl_sync(0xffffffffu, pB, 3, 4);
+        int wA = candA + pA - nA, wB = candB + pB - nB;
+        if (nA + nB > 0) {
+          float* sA_ = okA ? a.cand_score + (size_t)rowA * a.cand_cap + (size_t)split * a.seg_cap : nullptr;
+          int* iA_ = okA ? a.cand_item + (size_t)rowA * a.cand_cap + (size_t)split * a.seg_cap : nullptr;
+          float* sB_ = okB ? a.cand_score + (size_t)rowB * a.cand_cap + (size_t)split * a.seg_cap : nullptr;
+          int* iB_ = okB ? a.cand_item + (size_t)rowB * a.cand_cap + (size_t)split * a.seg_cap : nullptr;
+#pragma unroll
+          for (int j = 0; j < 64; ++j) {
+            const int item = item0 + 8 * (j >> 2) + col0 + (j & 1);
+            const bool in = full_tile || item < a.n_items;
+            if ((j >> 1) & 1) {
+              if (okB && in && d[j] >= thB) {
+                if (wB < a.seg_cap) { sB_[wB] = d[j]; iB_[wB] = item; }
+                ++wB;
+              }
+            } else if (okA && in && d[j] >= thA) {
+              if (wA < a.seg_cap) { sA_[wA] = d[j]; iA_[wA] = item; }
+              ++wA;
+            }
+          }
+        }
+        candA += totA;
+        candB += totB;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 64; ++j) {
+        const int item = item0 + 8 * (j >> 2) + col0 + (j & 1);
+        const bool rB = (j >> 1) & 1;
+        if ((rB ? okB : okA) && (full_tile || item < a.n_items))
+          a.out_scores[(size_t)(rB ? rowB : rowA) * a.out_ld + item] = d[j];
+      }
+    }
+  }
+  if (MODE == 2 && (lane & 3) == 0) {
+    if (okA) a.cand_count[(size_t)rowA * a.n_splits + split] = candA;
+    if (okB) a.cand_count[(size_t)rowB * a.n_splits + split] = candB;
   }
 }
 
@@ -403,14 +380,14 @@ extern "C" int fps_topk_mma(TopkArgs* args_in, const float* item_table, int id_b
   if (stages > TK_MAX_STAGES) stages = TK_MAX_STAGES;
   if (stages < 2) return -1003;
   a.n_stages = stages;
-  const size_t smem = blk * (MBv + stages) + 16 * 8 + 16 + 1024;
+  const size_t smem = blk * (MBv + stages) + 2 * TK_MAX_STAGES * 8 + 1024;
   const int grid = qblocks * a.n_splits;
 #define TK_LAUNCH2(IDT, MODE, MBT)                                                                 \
   do {                                                                                             \
     cudaError_t e = cudaFuncSetAttribute(fps_topk_mma_kernel<IDT, MODE, MBT>,                      \
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  \
     if (e != cudaSuccess) return (int)e;                                                           \
-    fps_topk_mma_kernel<IDT, MODE, MBT><<<grid, 128 + 128 * MBT, smem, stream>>>(map, a);          \
+    fps_topk_mma_kernel<IDT, MODE, MBT><<<grid, 256 * MBT + 32, smem, stream>>>(map, a);           \
   } while (0)
 #define TK_LAUNCH(IDT, MODE)                                                                       \
   do {                                                                                             \

@@ -1,4 +1,4 @@
-"""ctypes bindings for ``libfps_kernels.so`` (hand-written sm_100a kernels + fabric).
+"""ctypes bindings for ``libfps_kernels.so`` (hand-written sm_90a kernels + fabric).
 
 Every wrapper takes torch CUDA tensors, validates them, and launches on the *current* torch
 CUDA stream, so launches compose with torch streams, events and CUDA-graph capture.  There is
@@ -248,7 +248,7 @@ def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
 
     ``kernel="reg"`` (default): register-staged loads at full occupancy (csrc/fps_core.cu);
     ``kernel="tma"``: warp-specialised TMA/mbarrier pipeline (csrc/fps_mf_tma.cu) -- slower for
-    256-byte rows, kept for large rows (measurements: profiles/mf_fused_history.md).
+    256-byte rows, kept for large rows.
     ``items=None`` means ``users`` holds packed64 records (see :func:`pack_ratings`)."""
     _req(users, "users")
     user_sharded = isinstance(user_table, ShardTableC)
@@ -744,7 +744,7 @@ def topk_mma(items: torch.Tensor, mode: int, *, q_ids: Optional[torch.Tensor] = 
              theta: Optional[torch.Tensor] = None, cand_count: Optional[torch.Tensor] = None,
              cand_score: Optional[torch.Tensor] = None, cand_item: Optional[torch.Tensor] = None,
              tile_lo: int = 0, tile_limit: Optional[torch.Tensor] = None) -> None:
-    """tcgen05 scoring kernel (K6): queries (pulled from ``q_tab`` by id, or ``q_local``) x local
+    """wgmma scoring kernel (K6): queries (pulled from ``q_tab`` by id, or ``q_local``) x local
     ``items`` with a mode-dependent epilogue.  Only tiles ``tile_lo <= t < min(n_tiles, tile_limit[0])``
     are scored (``tile_limit``: optional int32 device scalar).  Mode 2 fills per-split candidate
     segments: ``cand_count`` is ``[n_q, n_splits]`` (see :func:`topk_geometry`).  csrc/fps_topk_mma.cu."""

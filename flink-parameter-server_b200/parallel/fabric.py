@@ -1,7 +1,7 @@
 """Symmetric-heap fabric over NVLink/NVSwitch.
 
 Each PS rank owns one device allocation; all ranks map all allocations, so a kernel running on
-any GPU can address any shard by pointer.  This is the B200-native replacement of the
+any GPU can address any shard by pointer.  This is the GPU-native replacement of the
 reference's ``partitionCustom`` + Flink network stack (FPS:416-420, 455-463) and of its
 iteration feedback edge (FPS:477-480): a pull is a peer load, a push is a peer reduction.
 

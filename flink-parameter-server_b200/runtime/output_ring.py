@@ -7,7 +7,8 @@ The fused kernel writes ``(id, vector)`` records into a device staging area; aft
 records into a ring in pinned host memory and publishes the new tail with a system-scope release store.
 ``poll()`` reads whatever has been published -- a plain host memory read, no stream synchronisation --
 and hands back ``(ids, vectors)``; ``records()`` yields ``Left((id, vector))`` like the host tier.
-``every=n`` samples one update in ``n`` (the full stream is ~1.8 TB/s at benchmark rates)."""
+``every=n`` samples one update in ``n`` (the full stream, one row per update at benchmark rates, is far
+more than the host link carries)."""
 from __future__ import annotations
 
 from typing import Iterator, List, Optional, Tuple

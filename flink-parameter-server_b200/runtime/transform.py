@@ -18,7 +18,7 @@ The returned :class:`ResultStream` is the ``DataStream[Either[WOut, PSOut]]`` of
 ``Left`` = worker outputs, ``Right`` = PS outputs.
 
 Backends: ``backend="local"`` runs the callbacks on the in-process asynchronous engine (host
-tier); declarative device logics (``runtime.device_engine``) run on the B200 fused tier.
+tier); declarative device logics (``runtime.device_engine``) run on the fused GPU tier.
 """
 from __future__ import annotations
 

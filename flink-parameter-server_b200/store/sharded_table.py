@@ -1,4 +1,4 @@
-"""Device-resident sharded parameter table (the B200-native "parameter server").
+"""Device-resident sharded parameter table (the GPU-native "parameter server").
 
 One dense fp32 block ``[rows_per_shard, stride]`` per PS rank lives in that GPU's HBM inside a
 :class:`SymmetricHeap`; every rank maps every shard, and kernels address rows through the

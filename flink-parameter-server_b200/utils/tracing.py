@@ -53,15 +53,16 @@ def measured_peaks() -> Dict[str, float]:
         with open(path) as f:
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 rate -- ceilings, not measurements
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "H100 SXM data sheet"}
 
 
 def roofline(bytes_moved: float, flops: float, ms: float, nvlink_bytes: float = 0.0) -> Dict[str, float]:
-    """Achieved / bound for a kernel: bound = slowest of HBM bytes, NVLink bytes (770 GB/s/dir) and
-    tensor FLOPs at the measured peaks."""
+    """Achieved / bound for a kernel: bound = slowest of HBM bytes, NVLink bytes (450 GB/s/dir,
+    the NVLink 4 data-sheet rate of an H100 SXM) and tensor FLOPs at the peaks of :func:`measured_peaks`."""
     p = measured_peaks()
     t_hbm = bytes_moved / (p["hbm_gbs"] * 1e9)
-    t_link = nvlink_bytes / 770e9
+    t_link = nvlink_bytes / 450e9
     t_flop = flops / (p["bf16_tflops"] * 1e12)
     bound = max(t_hbm, t_link, t_flop)
     return {"ms": ms, "bound_ms": bound * 1e3, "fraction_of_roofline": bound * 1e3 / ms if ms > 0 else 0.0,

@@ -1,4 +1,4 @@
-"""tcgen05 top-K scoring kernel vs fp32 PyTorch (TF32 tolerance) and brute-force top-K."""
+"""wgmma top-K scoring kernel vs fp32 PyTorch (TF32 tolerance) and brute-force top-K."""
 import pytest
 import torch
 

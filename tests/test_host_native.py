@@ -28,7 +28,7 @@ def test_native_interner():
 
 
 def test_kernel_library_builds_and_is_current():
-    """nvcc cross-compiles every kernel for sm_100a (no GPU needed); a stale or broken build fails here."""
+    """nvcc cross-compiles every kernel for sm_90a (no GPU needed); a stale or broken build fails here."""
     from fps_b200.ops import build
 
     path = build.build_kernels()          # rebuilds when sources changed; raises on compile errors
