@@ -154,6 +154,47 @@ def _seen_filter(rows, K: int, memory: int):
     return out
 
 
+class _SeenWindow:
+    """The per-user recent-item state of :func:`_seen_filter`, kept across micro-batches so the device
+    top-K can exclude the seen items exactly instead of over-fetching and filtering afterwards.  Same
+    ``(set, deque)`` bookkeeping, including its quirk: an item rated twice inside the window leaves the
+    set when its older copy leaves the window."""
+
+    def __init__(self, memory: int):
+        self.memory = int(memory)
+        self.seen, self.order = {}, {}
+
+    def exclusions(self, users, items):
+        """For a micro-batch ``(users, items)`` in stream order: the items each rating's list must not
+        contain (the user's set *before* that rating, so earlier ratings of the same batch count), as a
+        CSR ``(offsets int64 [n + 1], item ids int64)`` of numpy arrays; then advance the state past the
+        batch.  Each set is copied by numpy, O(|set|) per rating without a per-item Python loop."""
+        import numpy as np
+        from collections import deque
+
+        lens = np.zeros(len(users) + 1, dtype=np.int64)
+        parts = []
+        for j, (user, item) in enumerate(zip(users, items)):
+            s = self.seen.setdefault(user, set())
+            if s:
+                parts.append(np.fromiter(s, dtype=np.int64, count=len(s)))
+                lens[j + 1] = len(s)
+            s.add(item)
+            q = self.order.setdefault(user, deque())
+            q.append(item)
+            if self.memory > -1 and len(q) > self.memory:
+                s.discard(q.popleft())
+        ids = np.concatenate(parts) if parts else np.zeros(0, dtype=np.int64)
+        return np.cumsum(lens), ids
+
+    def device_exclusions(self, users, items, dev):
+        """:meth:`exclusions` as device tensors, or ``None`` when no rating of the batch excludes anything."""
+        off, ids = self.exclusions(users, items)
+        if ids.size == 0:
+            return None
+        return torch.from_numpy(off).to(dev), torch.from_numpy(ids).to(dev)
+
+
 def ps_topk_generator_device(src, model, K: int = 100, workerK: int = 75, userMemory: int = 0,
                              batch_size: int = 4096, group=None, sort_by_length: bool = True):
     """Top-K serving over a pre-trained model on the device tier (capability of ``psTopKGenerator``,
@@ -201,20 +242,22 @@ def ps_topk_generator_device(src, model, K: int = 100, workerK: int = 75, userMe
 
         serving.local = DeviceTopK(local, sort_by_length=True)
     ratings = list(src.collect() if hasattr(src, "collect") else src)
-    want = K + (min(userMemory, 4 * K) if userMemory >= 0 else 4 * K)   # room for the seen-item filter
+    window = _SeenWindow(userMemory) if userMemory != 0 else None    # seen items are excluded on the device
     rows = []
     for a in range(0, len(ratings), batch_size):
         chunk = ratings[a:a + batch_size]
         q = torch.tensor([min(max(r.user, 0), n_users - 1) for r in chunk], dtype=torch.int64, device=dev)
         known = (table.pull(q)[:, k] == 1.0).cpu().tolist()
-        sc, ids = serving.topk(q, want, workerK=max(workerK, want))
+        exclude = None if window is None else \
+            window.device_exclusions([r.user for r in chunk], [r.item for r in chunk], dev)
+        sc, ids = serving.topk(q, K, workerK=max(workerK or K, K), exclude=exclude)
         sc, ids = sc.cpu().tolist(), ids.cpu().tolist()
         for j, r in enumerate(chunk):
             ok = known[j] and 0 <= r.user < n_users
             cand = [(s, i) for s, i in zip(sc[j], ids[j]) if i >= 0 and s > -1.0e38] if ok else []
-            rows.append((r.user, r.item, r.getEventTime(), cand))
+            rows.append((r.item, r.getEventTime(), cand))
     table.close()
-    return [(item, ts, topk) for (_u, item, ts, topk) in _seen_filter(rows, K, userMemory)]
+    return rows
 
 
 class _LearnerModel:
@@ -248,7 +291,8 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
     1. every rank scores the batch's users -- pulled from the PS by the wgmma kernel's A-gather --
        against ITS item partition (``fps_topk_mma``) and keeps ``workerK`` candidates;
     2. the partial lists travel to the merge rank as one-sided stores (:class:`P2PGather`) and are
-       merged by ``fps_row_topk`` (``CollectTopKFromEachWorker.scala:41-56``; seen-item filter on the host);
+       merged by ``fps_row_topk`` (``CollectTopKFromEachWorker.scala:41-56``); the user's last
+       ``userMemory`` items are excluded exactly inside the device top-K (per-query exclusion lists);
     3. the OWNER of each rated item trains: its local item row is updated in place and the user delta is
        pushed to the PS (``...AndTopKGeneratorWorker.scala:128-164``) -- the fused MF kernel with the
        roles swapped (worker-local rows = items, PS rows = users), negatives drawn from the owner's items.
@@ -282,8 +326,8 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
     stats = torch.zeros(2, dtype=torch.float32, device=dev)
     nan_flag = torch.zeros(1, dtype=torch.int32, device=dev)
     err_mode = ERR_PLAIN if plain_residual else ERR_SIGMOID
-    want = K + (min(userMemory, 4 * K) if userMemory >= 0 else K)
-    wk = max(workerK or 0, want)
+    wk = max(workerK or K, K)
+    window = _SeenWindow(userMemory) if userMemory != 0 else None    # same state on every rank
     gen = torch.Generator(device=dev).manual_seed(seed * 7919 + 13)
     rows = []
     users.barrier()
@@ -295,7 +339,9 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
         i = torch.tensor([r.item for r in chunk], dtype=torch.int32, device=dev)
         rt = torch.tensor([r.rating for r in chunk], dtype=torch.float32, device=dev)
         # 1 + 2: local top-workerK of every query on this rank's items, gathered + merged on rank 0
-        sc, ids = serving.topk(u.long(), want, workerK=wk, dst=0)
+        exclude = None if window is None else \
+            window.device_exclusions([r.user for r in chunk], [r.item for r in chunk], dev)
+        sc, ids = serving.topk(u.long(), K, workerK=wk, dst=0, exclude=exclude)
         if sc is not None:
             sc, ids = sc.cpu().tolist(), ids.cpu().tolist()
             for j, r in enumerate(chunk):
@@ -325,7 +371,7 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
         from ...errors import FactorIsNotANumberException
 
         raise FactorIsNotANumberException("non-finite SGD update")
-    out = _ListWithModel(_seen_filter(rows, K, userMemory) if rank == 0 else [])
+    out = _ListWithModel(rows if rank == 0 else [])
     out.users, out.items, out.item_ids, out.n_items = users, items, local_ids, n_valid
     out.model = _LearnerModel(users, items, world, rank, numFactors)
     if getattr(serving, "_p2p_gather", None) is not None:

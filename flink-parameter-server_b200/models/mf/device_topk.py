@@ -13,6 +13,17 @@ Algorithm (exact, tile-pruned -- the GPU-idiomatic replacement of the LEMP bucke
   select  top-K of the candidates.
 Scores are TF32 products accumulated in FP32; ``rescore=True`` recomputes the K winners in full
 FP32 (ordering among near-ties may then differ from the TF32 ranking by < 1e-3 relative).
+
+Per-query exclusion (``topk(..., exclude=...)``, the seen-item filter of CollectTopKFromEachWorker):
+let ``E_q`` be the number of distinct excluded items of query ``q`` present in the table.  The
+``(K + E_q)``-th largest tile maximum is still a lower bound of the K-th best *admissible* score:
+those ``K + E_q`` tiles hold ``K + E_q`` distinct items scoring at least that much, and at most ``E_q``
+of them are excluded.  The same argument holds for the LENGTH-pruned ``theta0`` (prefix of the
+table) and for the overflow tightening (the ``(K + E_q)``-th best kept candidate); the tile count of
+``_tiles_needed`` follows from theta unchanged.  When ``K + E_q`` exceeds the tiles scored, theta is
+-3e38: the row overflows into the brute-force fallback (excluded columns masked), so the result stays
+exact.  Excluded candidates are dropped in the select stage (``fps_row_topk``); the scoring kernel
+is not involved.
 """
 from __future__ import annotations
 
@@ -22,6 +33,33 @@ import torch
 
 from ...ops import native
 from ...store.sharded_table import ShardedTable
+
+
+def normalize_exclude(offsets, rows, n_q: int, n_items: int, inv_perm: Optional[torch.Tensor] = None,
+                      device=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Per-query exclusion CSR in the caller's row numbering -> the form ``fps_row_topk`` reads.
+
+    ``offsets`` [n_q + 1] and ``rows`` may be unsorted within a query and hold duplicates or values
+    outside ``[0, n_items)`` (ignored).  Rows are mapped through ``inv_perm`` (caller row -> table
+    position) when given, then sorted and de-duplicated per query with one sort on ``query * n_items +
+    position`` keys.  Returns ``(offsets int32 [n_q + 1], positions int32 [E], counts int32 [n_q])`` on
+    ``device`` (default: the device of ``rows``).  Plain torch ops, no host loop."""
+    dev = torch.device(device) if device is not None else torch.as_tensor(rows).device
+    off = torch.as_tensor(offsets).to(dev, torch.int64).reshape(-1)
+    r = torch.as_tensor(rows).to(dev, torch.int64).reshape(-1)
+    if off.numel() != n_q + 1:
+        raise ValueError(f"exclude offsets must have n_q + 1 = {n_q + 1} entries, got {off.numel()}")
+    j = torch.arange(r.numel(), device=dev)
+    q = torch.searchsorted(off[1:].contiguous(), j, right=True)        # query of entry j
+    keep = (j >= off[0]) & (q < n_q) & (r >= 0) & (r < n_items)
+    q, r = q[keep], r[keep]
+    if inv_perm is not None:
+        r = inv_perm[r]
+    key = torch.unique_consecutive(torch.sort(q * n_items + r).values)
+    cnt = torch.bincount(key // n_items, minlength=n_q)
+    out_off = torch.zeros(n_q + 1, dtype=torch.int64, device=dev)
+    out_off[1:] = torch.cumsum(cnt, 0)
+    return out_off.to(torch.int32), (key % n_items).to(torch.int32), cnt.to(torch.int32)
 
 
 class DeviceTopK:
@@ -38,10 +76,12 @@ class DeviceTopK:
                  pass1_fraction: Optional[float] = None):
         if items.dim() != 2 or items.shape[1] % 4 != 0:
             raise ValueError("items must be [n_items, stride] with stride % 4 == 0")
-        self.perm = None
+        self.perm = self.inv_perm = None
         if sort_by_length:
             lens = items.norm(dim=1)
             self.perm = torch.argsort(lens, descending=True)
+            self.inv_perm = torch.empty_like(self.perm)
+            self.inv_perm[self.perm] = torch.arange(self.perm.numel(), device=self.perm.device)
             items = items[self.perm].contiguous()
             self.tile_maxlen = lens[self.perm][:: native.TOPK_TILE].contiguous()
         self.items = items
@@ -56,6 +96,7 @@ class DeviceTopK:
             pass1_fraction = 0.125 if self.n_tiles >= 512 else 0.0
         self.pass1_fraction = pass1_fraction
         self._last = (0, None, None)
+        self.last_fallback_rows = 0       # rows the last ``topk`` answered by brute force (overflow)
         self.trace = None                 # set to [] to collect (stage, ms) pairs (synchronising!)
         self._t0 = None
 
@@ -100,36 +141,56 @@ class DeviceTopK:
         return out
 
     def topk(self, K: int, *, q_ids=None, q_table: Optional[ShardedTable] = None, q_local=None,
-             rescore: bool = False) -> Tuple[torch.Tensor, torch.Tensor]:
+             rescore: bool = False, exclude=None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Returns ``(scores [n_q, K'], item_rows [n_q, K'])`` best first, ``K' = min(K, n_items)``;
-        item_rows index the caller's item table."""
+        item_rows index the caller's item table.
+
+        ``exclude=(offsets, rows)``: items query ``q`` must not get, ``rows[offsets[q]:offsets[q+1]]``
+        in the caller's row numbering (see :func:`normalize_exclude`).  The result is the exact top-K
+        of the remaining items; a query with fewer than ``K'`` of them gets ``(-3e38, -1)`` entries at
+        the end."""
         n_q = q_ids.numel() if q_ids is not None else q_local.shape[0]
         Kp = min(K, self.n_items)
         if Kp > 2048:
             raise ValueError("DeviceTopK supports K <= 2048 (shared-memory sort buffer of fps_row_topk)")
         T = native.TOPK_TILE
         dev = self.items.device
+        ex = None
+        Ke = Kp                              # K plus the largest per-query exclusion count
+        if exclude is not None:
+            ex_off, ex_pos, ex_cnt = normalize_exclude(exclude[0], exclude[1], n_q, self.n_items,
+                                                       self.inv_perm, device=dev)
+            if ex_pos.numel() > 0:
+                host = torch.cat([ex_off, ex_cnt.max().reshape(1)]).cpu()    # one transfer: offsets + max E_q
+                ex = host[:-1]
+                Ke = Kp + int(host[-1])
         # candidate buffer: a few x K per query is typical (worst case K*128 and more with ties); an
         # overflowing row raises its theta and repeats pass 2 instead of growing the buffer
-        cap = min(max(2048, 16 * Kp), max(T, (self.n_items + T - 1) // T * T) * 2)
+        cap = min(max(2048, 16 * Ke), max(T, (self.n_items + T - 1) // T * T) * 2)
         per_row = self.n_tiles * 4 + cap * 8
         chunk = max(256, (self.max_batch_bytes // per_row) // 256 * 256)
         tab = q_table.table_c if q_table is not None else None
         outs, outi = [], []
+        self.last_fallback_rows = 0
         for a in range(0, n_q, chunk):
             b = min(n_q, a + chunk)
             ids = q_ids[a:b].contiguous() if q_ids is not None else None
             ql = q_local[a:b].contiguous() if q_local is not None else None
             n = b - a
+            kq = c_ex = None                 # per-query K + E_q, and the chunk's exclusion CSR
+            if ex is not None:
+                e0, e1 = int(ex[a]), int(ex[b])
+                c_ex = ((ex_off[a:b + 1] - e0).contiguous(), ex_pos[e0:e1])
+                kq = (ex_cnt[a:b] + Kp).contiguous()
             self._mark("start")
             kw = dict(q_ids=ids, q_tab=tab, q_local=ql)
             # ---- pass 1: per-(query, tile) maxima ------------------------------------------------
             lim1 = lim2 = None
             p1 = self.n_tiles
-            prune = self.perm is not None and self.n_tiles >= 16 and max(Kp, self.n_tiles // 8) < self.n_tiles
+            prune = self.perm is not None and self.n_tiles >= 16 and max(Ke, self.n_tiles // 8) < self.n_tiles
             frac_tiles = 0
             if not prune and self.pass1_fraction:
-                frac_tiles = max(Kp, int(self.n_tiles * float(self.pass1_fraction)))
+                frac_tiles = max(Ke, int(self.n_tiles * float(self.pass1_fraction)))
             if not prune and 0 < frac_tiles < self.n_tiles:
                 p1 = frac_tiles
                 tile_max = torch.full((n, self.n_tiles), -3.0e38, dtype=torch.float32, device=dev)
@@ -145,16 +206,16 @@ class DeviceTopK:
                 # maximum already bounds how far down the length-sorted table a top-K item can sit.
                 q = q_table.pull(ids) if ids is not None else ql
                 qnorm = q.norm(dim=1)
-                p1 = max(Kp, self.n_tiles // 8)
+                p1 = max(Ke, self.n_tiles // 8)
                 tile_max = torch.full((n, self.n_tiles), -3.0e38, dtype=torch.float32, device=dev)
                 first = torch.full((1,), p1, dtype=torch.int32, device=dev)
                 native.topk_mma(self.items, 1, tile_max=tile_max, tile_limit=first, **kw)
                 self._mark("pass1a")
-                theta0 = native.row_kth_largest(tile_max, Kp, n_cols=p1)
+                theta0 = native.row_kth_largest(tile_max, Kp, n_cols=p1, k_per_row=kq)
                 lim1 = self._tiles_needed(theta0, qnorm)
                 native.topk_mma(self.items, 1, tile_max=tile_max, tile_lo=p1, tile_limit=lim1, **kw)
                 self._mark("pass1b")
-            theta = native.row_kth_largest(tile_max, Kp)     # -3e38 when there are fewer than K tiles
+            theta = native.row_kth_largest(tile_max, Kp, k_per_row=kq)  # -3e38 with fewer than K (+E_q) tiles
             if prune:
                 lim2 = self._tiles_needed(theta, qnorm)       # <= tiles scored in pass 1 (theta >= theta0)
             self._mark("theta")
@@ -176,17 +237,18 @@ class DeviceTopK:
                     bad = torch.nonzero(over).flatten()
                     break
                 # K-th best of the candidates that were kept: a valid, higher lower bound
-                theta = torch.maximum(theta, native.row_kth_largest(cs, Kp))
+                theta = torch.maximum(theta, native.row_kth_largest(cs, Kp, k_per_row=kq))
                 if prune:
                     lim2 = torch.minimum(lim2, self._tiles_needed(theta, qnorm))
                 self._mark("tighten")
             self._last = (p1, lim1, lim2)
-            sc, rows = native.row_topk(cs, ci, Kp)               # select + sort, one CTA per row
+            sc, rows = native.row_topk(cs, ci, Kp, exclude=c_ex)  # select + sort, one CTA per row
             self._mark("select")
             rows = rows.to(torch.int64)
             if bad is not None:
                 # rows that still overflow (e.g. thousands of items tied at theta, an all-zero query):
                 # brute force, always exact
+                self.last_fallback_rows += bad.numel()
                 bq = dict(q_ids=ids[bad].contiguous(), q_tab=tab) if ids is not None else \
                     dict(q_local=ql[bad].contiguous())
                 for s0 in range(0, bad.numel(), 64):
@@ -194,18 +256,41 @@ class DeviceTopK:
                     full = torch.empty((sel.numel(), self.n_items), dtype=torch.float32, device=dev)
                     sub = {k: (v[s0:s0 + 64].contiguous() if torch.is_tensor(v) else v) for k, v in bq.items()}
                     native.topk_mma(self.items, 0, out_scores=full, **sub)
+                    if c_ex is not None:
+                        _mask_excluded(full, sel, n, *c_ex)
                     top = torch.topk(full, Kp, dim=1)
                     sc[sel], rows[sel] = top.values, top.indices
+            if c_ex is not None:
+                # fewer than K admissible items: unused candidate slots / masked columns won
+                short = sc < -1.0e38
+                sc, rows = sc.masked_fill(short, -3.0e38), rows.masked_fill(short, -1)
             if rescore:
                 q = (q_table.pull(ids) if ids is not None else ql[:, : self.stride])
                 q = torch.nn.functional.pad(q, (0, self.stride - q.shape[1]))
-                exact = torch.einsum("qd,qkd->qk", q, self.items[rows])
+                if c_ex is None:
+                    exact = torch.einsum("qd,qkd->qk", q, self.items[rows])
+                else:
+                    exact = torch.einsum("qd,qkd->qk", q, self.items[rows.clamp_min(0)])
+                    exact = exact.masked_fill(rows < 0, -3.0e38)
                 order = torch.argsort(exact, dim=1, descending=True)
                 sc, rows = torch.gather(exact, 1, order), torch.gather(rows, 1, order)
-            if self.perm is not None:
-                rows = self.perm[rows]      # back to row numbers of the caller's (unsorted) table
+            if self.perm is not None:       # back to row numbers of the caller's (unsorted) table
+                rows = self.perm[rows] if c_ex is None else \
+                    torch.where(rows >= 0, self.perm[rows.clamp_min(0)], rows)
             outs.append(sc); outi.append(rows)
         return torch.cat(outs), torch.cat(outi)
+
+
+def _mask_excluded(full: torch.Tensor, sel: torch.Tensor, n: int, off: torch.Tensor, pos: torch.Tensor) -> None:
+    """Brute-force fallback: set the excluded columns of the chunk rows ``sel`` (rows of ``full``) to
+    -inf.  ``off`` / ``pos``: the chunk's exclusion CSR over ``n`` rows, table positions."""
+    q = torch.repeat_interleave(torch.arange(n, device=full.device), (off[1:] - off[:-1]).long(),
+                                output_size=pos.numel())
+    slot = torch.full((n,), -1, dtype=torch.int64, device=full.device)
+    slot[sel] = torch.arange(sel.numel(), device=full.device)
+    m = slot[q]
+    hit = m >= 0
+    full[m[hit], pos[hit].long()] = float("-inf")
 
 
 def merge_partial_topk(scores: torch.Tensor, items: torch.Tensor, K: int,
@@ -240,6 +325,7 @@ class DistributedTopK:
         self.users, self.group = user_table, group
         self.local = DeviceTopK(local_items)
         self.item_ids = local_item_ids.to(torch.int64)
+        self._ids_sorted, self._ids_order = torch.sort(self.item_ids)   # global id -> local row lookup
         self.world = dist.get_world_size(group) if (dist.is_available() and dist.is_initialized()) else 1
 
     def _gather_lists(self, sc: torch.Tensor, gids: torch.Tensor, dst):
@@ -249,12 +335,22 @@ class DistributedTopK:
 
         return gather_pair(self, sc, gids, dst, self.group, self.users.device)
 
-    def topk(self, query_user_ids: torch.Tensor, K: int, workerK: Optional[int] = None, dst=None):
+    def topk(self, query_user_ids: torch.Tensor, K: int, workerK: Optional[int] = None, dst=None,
+             exclude=None):
         """``dst=None``: every rank gets the merged lists; ``dst=r``: only rank ``r`` merges (the
-        parallelism-1 sink of CollectTopKFromEachWorker.scala:41-56), the others return ``(None, None)``."""
+        parallelism-1 sink of CollectTopKFromEachWorker.scala:41-56), the others return ``(None, None)``.
+        ``exclude=(offsets, ids)``: per-query CSR of **global item ids** no list may contain; every rank
+        drops the ids it does not own, so each partial list is already filtered and the merge is the
+        plain one.  Lists with fewer admissible items than ``K`` end in ``(-3e38, -1)`` entries."""
         wk = min(workerK or K, self.local.n_items)
-        sc, rows = self.local.topk(wk, q_ids=query_user_ids, q_table=self.users)
-        gids = self.item_ids[rows]
+        ex = None
+        if exclude is not None:
+            g = torch.as_tensor(exclude[1]).to(self.item_ids.device, torch.int64).reshape(-1)
+            at = torch.searchsorted(self._ids_sorted, g).clamp_max(self._ids_sorted.numel() - 1)
+            ex = (exclude[0], torch.where(self._ids_sorted[at] == g, self._ids_order[at], -1))
+        sc, rows = self.local.topk(wk, q_ids=query_user_ids, q_table=self.users, exclude=ex)
+        gids = self.item_ids[rows] if ex is None else \
+            torch.where(rows >= 0, self.item_ids[rows.clamp_min(0)], -1)
         if self.world == 1:
             return merge_partial_topk(sc, gids, K)
         if wk < (workerK or K):  # pad so all ranks contribute equally sized lists

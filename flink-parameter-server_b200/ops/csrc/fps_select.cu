@@ -5,6 +5,12 @@
 //   fps_row_topk  : sorted top-K (score, item) of every row's candidate list / concatenated partial
 //                   lists (CollectTopKFromEachWorker.scala:41-56 without the host round trip)
 //
+// Both take optional per-row arguments for the seen-item filter of the generators: fps_row_kth a
+// per-row k (the (K + E_q)-th tile maximum is the bound when E_q items of row q are excluded), and
+// fps_row_topk an exclusion list per row in CSR form (offsets [n_rows+1], items sorted and
+// de-duplicated within each row).  An excluded candidate is found by binary search and never enters
+// the radix select or the sort; the plain instantiation of fps_row_topk is the code without the lookup.
+//
 // One CTA per row.  Selection is an MSD radix select over order-preserving 32-bit keys (4 passes of 8
 // bits, per-warp shared-memory histograms), so the cost is O(n) per row regardless of K -- torch.topk
 // on the same shapes was the largest term of the top-K pipeline (profiles/topk_mma.md).  The final
@@ -25,8 +31,9 @@ __device__ __forceinline__ float sel_unkey(uint32_t k) {
   return __uint_as_float(u);
 }
 
-// Key of the k-th largest (k is 1-based, 1 <= k <= n) of src[0..n).  Block-wide; all threads return it.
-__device__ uint32_t sel_block_kth_key(const float* src, int n, int k, uint32_t* hist /*[SEL_WARPS*256]*/,
+// Key of the k-th largest (k is 1-based, 1 <= k <= n) of key_at(0..n).  Block-wide; all threads return it.
+template <class KeyAt>
+__device__ uint32_t sel_block_kth_key(KeyAt key_at, int n, int k, uint32_t* hist /*[SEL_WARPS*256]*/,
                                       uint32_t* bcast /*[2]*/) {
   uint32_t prefix = 0, mask = 0;
   uint32_t krem = (uint32_t)k;
@@ -35,7 +42,7 @@ __device__ uint32_t sel_block_kth_key(const float* src, int n, int k, uint32_t* 
     for (int i = threadIdx.x; i < SEL_WARPS * 256; i += SEL_THREADS) hist[i] = 0;
     __syncthreads();
     for (int i = threadIdx.x; i < n; i += SEL_THREADS) {
-      const uint32_t key = sel_key(src[i]);
+      const uint32_t key = key_at(i);
       if ((key & mask) == prefix) atomicAdd(&hist[warp * 256 + ((key >> shift) & 0xFFu)], 1u);
     }
     __syncthreads();
@@ -82,16 +89,43 @@ __device__ uint32_t sel_block_kth_key(const float* src, int n, int k, uint32_t* 
   return prefix;
 }
 
+__device__ __forceinline__ uint32_t sel_block_kth_key(const float* src, int n, int k, uint32_t* hist,
+                                                      uint32_t* bcast) {
+  return sel_block_kth_key([src](int i) { return sel_key(src[i]); }, n, k, hist, bcast);
+}
+
+// Is `item` in the sorted list ex[0..n)?  (lower_bound)
+__device__ __forceinline__ bool sel_excluded(const int* __restrict__ ex, int n, int item) {
+  const int* end = ex + n;
+  while (n > 0) {
+    const int half = n >> 1;
+    if (__ldg(ex + half) < item) {
+      ex += half + 1;
+      n -= half + 1;
+    } else {
+      n = half;
+    }
+  }
+  return ex < end && __ldg(ex) == item;
+}
+
+// Key 0 sorts below every float key (only the NaN bit pattern 0xFFFFFFFF maps to it): an excluded
+// candidate gets it, so it can only be "selected" when a row has fewer than K admissible candidates,
+// and the gather passes below skip it.
+#define SEL_KEY_EXCLUDED 0u
+
 __global__ void __launch_bounds__(SEL_THREADS)
     fps_row_kth_kernel(const float* __restrict__ x, long long ld, int n_cols,
-                       const int* __restrict__ counts, int K, int staged, float* __restrict__ out) {
+                       const int* __restrict__ counts, int K, const int* __restrict__ k_per_row, int staged,
+                       float* __restrict__ out) {
   extern __shared__ float sel_row[];
   __shared__ uint32_t hist[SEL_WARPS * 256];
   __shared__ uint32_t bcast[2];
   const long long row = blockIdx.x;
   int n = n_cols;
   if (counts != nullptr) n = min(counts[row], n_cols);
-  if (n < K) {  // fewer than K values: no bound (uniform branch)
+  if (k_per_row != nullptr) K = k_per_row[row];
+  if (n < K || K < 1) {  // fewer than K values: no bound (uniform branch)
     if (threadIdx.x == 0) out[row] = -3.0e38f;
     return;
   }
@@ -105,9 +139,11 @@ __global__ void __launch_bounds__(SEL_THREADS)
   if (threadIdx.x == 0) out[row] = sel_unkey(key);
 }
 
+template <bool EXCL>
 __global__ void __launch_bounds__(SEL_THREADS)
     fps_row_topk_kernel(const float* __restrict__ cs, const int* __restrict__ ci, long long ld, int cap,
                         const int* __restrict__ counts, int K, int S, int staged,
+                        const int* __restrict__ ex_off, const int* __restrict__ ex_items, int ex_total,
                         float* __restrict__ out_s, int* __restrict__ out_i) {
   extern __shared__ __align__(16) unsigned char sel_dyn[];
   unsigned long long* sortbuf = reinterpret_cast<unsigned long long*>(sel_dyn);  // [S]
@@ -120,17 +156,32 @@ __global__ void __launch_bounds__(SEL_THREADS)
   if (counts != nullptr) n = min(counts[row], cap);
   const float* src = cs + row * ld;
   const int* items = ci + row * ld;
+  const int* ex = nullptr;
+  int n_ex = 0;
+  if (EXCL) {
+    // clamped into [0, ex_total]: a malformed CSR gives a wrong filter, never an out-of-bounds read
+    const int e0 = min(max(ex_off[row], 0), ex_total);
+    ex = ex_items + e0;
+    n_ex = min(max(ex_off[row + 1], e0), ex_total) - e0;
+  }
   for (int i = threadIdx.x; i < S; i += SEL_THREADS) sortbuf[i] = 0ull;
   if (threadIdx.x == 0) { n_gt = 0; n_eq = 0; }
   if (staged) {
-    for (int i = threadIdx.x; i < n; i += SEL_THREADS) stage[i] = src[i];
+    // an excluded candidate is staged as the float whose key is SEL_KEY_EXCLUDED: one search per candidate
+    for (int i = threadIdx.x; i < n; i += SEL_THREADS)
+      stage[i] = (EXCL && sel_excluded(ex, n_ex, items[i])) ? __uint_as_float(0xFFFFFFFFu) : src[i];
     src = stage;
   }
   __syncthreads();
+  // unstaged rows (cap > SEL_STAGE_MAX - 2S) search on every read instead
+  auto key_at = [=](int i) -> uint32_t {
+    if (EXCL && !staged && sel_excluded(ex, n_ex, items[i])) return SEL_KEY_EXCLUDED;
+    return sel_key(src[i]);
+  };
   uint32_t kth = 0;
-  if (n > K) kth = sel_block_kth_key(src, n, K, hist, bcast);
+  if (n > K) kth = sel_block_kth_key(key_at, n, K, hist, bcast);
   for (int i = threadIdx.x; i < n; i += SEL_THREADS) {
-    const uint32_t key = sel_key(src[i]);
+    const uint32_t key = key_at(i);
     if (key > kth) {  // at most K-1 of these when n > K, at most n <= K <= S otherwise
       const int slot = atomicAdd(&n_gt, 1);
       if (slot < S) sortbuf[slot] = ((unsigned long long)key << 32) | (0xFFFFFFFFu - (uint32_t)items[i]);
@@ -138,11 +189,14 @@ __global__ void __launch_bounds__(SEL_THREADS)
   }
   __syncthreads();
   const int base = min(n_gt, S);
-  for (int i = threadIdx.x; i < n; i += SEL_THREADS) {
-    const uint32_t key = sel_key(src[i]);
-    if (key == kth) {  // ties with the K-th score: as many as the sort buffer holds
-      const int slot = base + atomicAdd(&n_eq, 1);
-      if (slot < S) sortbuf[slot] = ((unsigned long long)key << 32) | (0xFFFFFFFFu - (uint32_t)items[i]);
+  // EXCL: kth == SEL_KEY_EXCLUDED means fewer than K admissible candidates, all taken by the pass above
+  if (!EXCL || kth != SEL_KEY_EXCLUDED) {
+    for (int i = threadIdx.x; i < n; i += SEL_THREADS) {
+      const uint32_t key = key_at(i);
+      if (key == kth) {  // ties with the K-th score: as many as the sort buffer holds
+        const int slot = base + atomicAdd(&n_eq, 1);
+        if (slot < S) sortbuf[slot] = ((unsigned long long)key << 32) | (0xFFFFFFFFu - (uint32_t)items[i]);
+      }
     }
   }
   __syncthreads();
@@ -166,10 +220,11 @@ __global__ void __launch_bounds__(SEL_THREADS)
   }
 }
 
+// k_per_row (optional, int32 [n_rows]) replaces K row by row.
 extern "C" int fps_row_kth(const float* x, long long ld, int n_rows, int n_cols, const int* counts,
-                           int K, float* out, cudaStream_t stream) {
+                           int K, const int* k_per_row, float* out, cudaStream_t stream) {
   if (n_rows <= 0) return 0;
-  if (K < 1) return -1201;
+  if (K < 1 && k_per_row == nullptr) return -1201;
   const int staged = n_cols <= SEL_STAGE_MAX ? 1 : 0;
   const size_t smem = staged ? (size_t)n_cols * sizeof(float) : 0;
   if (smem > 32 * 1024) {  // static (histograms) + dynamic must stay under 48 KB without the opt-in
@@ -177,24 +232,28 @@ extern "C" int fps_row_kth(const float* x, long long ld, int n_rows, int n_cols,
                                          (int)smem);
     if (e != cudaSuccess) return (int)e;
   }
-  fps_row_kth_kernel<<<n_rows, SEL_THREADS, smem, stream>>>(x, ld, n_cols, counts, K, staged, out);
+  fps_row_kth_kernel<<<n_rows, SEL_THREADS, smem, stream>>>(x, ld, n_cols, counts, K, k_per_row, staged, out);
   return (int)cudaGetLastError();
 }
 
+// ex_off / ex_items (optional, both or neither): per-row exclusion lists, CSR over ex_items[0..ex_total) with
+// each row's items sorted ascending (duplicates are harmless).  K <= 2048 bounds the output, not K plus the excluded count.
 extern "C" int fps_row_topk(const float* cs, const int* ci, long long ld, int n_rows, int cap,
-                            const int* counts, int K, float* out_s, int* out_i, cudaStream_t stream) {
+                            const int* counts, int K, const int* ex_off, const int* ex_items, int ex_total,
+                            float* out_s, int* out_i, cudaStream_t stream) {
   if (n_rows <= 0) return 0;
   if (K < 1 || K > 2048) return -1202;
+  if ((ex_off == nullptr) != (ex_items == nullptr)) return -1203;
   int S = 64;
   while (S < 2 * K) S <<= 1;
   const int staged = cap <= SEL_STAGE_MAX - 2 * S ? 1 : 0;
   const size_t smem = (size_t)S * 8 + (staged ? (size_t)cap * sizeof(float) : 0);
+  auto kern = ex_off != nullptr ? fps_row_topk_kernel<true> : fps_row_topk_kernel<false>;
   if (smem > 32 * 1024) {  // static (histograms) + dynamic must stay under 48 KB without the opt-in
-    cudaError_t e = cudaFuncSetAttribute(fps_row_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
   }
-  fps_row_topk_kernel<<<n_rows, SEL_THREADS, smem, stream>>>(cs, ci, ld, cap, counts, K, S, staged, out_s,
-                                                             out_i);
+  kern<<<n_rows, SEL_THREADS, smem, stream>>>(cs, ci, ld, cap, counts, K, S, staged, ex_off, ex_items, ex_total,
+                                              out_s, out_i);
   return (int)cudaGetLastError();
 }

@@ -790,37 +790,64 @@ def topk_mma(items: torch.Tensor, mode: int, *, q_ids: Optional[torch.Tensor] = 
 
 
 def row_kth_largest(x: torch.Tensor, K: int, counts: Optional[torch.Tensor] = None,
-                    n_cols: Optional[int] = None) -> torch.Tensor:
+                    n_cols: Optional[int] = None, k_per_row: Optional[torch.Tensor] = None) -> torch.Tensor:
     """K-th largest value of every row of ``x`` [n, L] (only the first ``n_cols`` columns if given);
-    rows with fewer than ``K`` valid entries (``counts[row] < K``) give -3e38.  Radix select,
-    csrc/fps_select.cu."""
+    rows with fewer than ``K`` valid entries (``counts[row] < K``) give -3e38.  ``k_per_row`` (int32
+    [n]) replaces ``K`` row by row.  Radix select, csrc/fps_select.cu."""
     _req(x, "x", torch.float32)
+    n = x.shape[0]
     if counts is not None:
         _req(counts, "counts", torch.int32)
-    out = torch.empty(x.shape[0], dtype=torch.float32, device=x.device)
+    if k_per_row is not None:
+        _req(k_per_row, "k_per_row", torch.int32)
+        if k_per_row.shape != (n,) or k_per_row.device != x.device:
+            raise ValueError(f"k_per_row must be [{n}] on {x.device}")
+    out = torch.empty(n, dtype=torch.float32, device=x.device)
     cols = int(x.shape[1] if n_cols is None else min(n_cols, x.shape[1]))
-    _check(lib().fps_row_kth(C.c_void_p(x.data_ptr()), C.c_longlong(x.stride(0)), int(x.shape[0]),
+    _check(lib().fps_row_kth(C.c_void_p(x.data_ptr()), C.c_longlong(x.stride(0)), int(n),
                              cols, C.c_void_p(counts.data_ptr() if counts is not None else None),
-                             int(K), C.c_void_p(out.data_ptr()), _stream()), "row_kth")
+                             int(K), C.c_void_p(k_per_row.data_ptr() if k_per_row is not None else None),
+                             C.c_void_p(out.data_ptr()), _stream()), "row_kth")
     _bump()
     return out
 
 
-def row_topk(scores: torch.Tensor, items: torch.Tensor, K: int, counts: Optional[torch.Tensor] = None):
+def row_topk(scores: torch.Tensor, items: torch.Tensor, K: int, counts: Optional[torch.Tensor] = None,
+             exclude: Optional[tuple] = None):
     """Sorted (descending) top-``K`` ``(score, item)`` of every row of the candidate arrays
     ``scores`` / ``items`` [n, cap] (int32 items); ``counts[row]`` limits the valid prefix.  Missing
-    entries are ``(-3e38, -1)``; equal scores are ordered by ascending item."""
+    entries are ``(-3e38, -1)``; equal scores are ordered by ascending item.  ``exclude=(offsets,
+    ex_items)``: int32 CSR, ``offsets`` [n + 1]; row ``r``'s excluded items ``ex_items[offsets[r]:
+    offsets[r+1]]`` must be sorted ascending (see ``models.mf.device_topk.normalize_exclude``).
+    Candidates whose item is excluded are dropped before the selection; rows left with fewer than ``K``
+    get the missing-entry tail.  The kernel clamps every offset into ``[0, len(ex_items)]``, so a
+    malformed CSR filters wrongly but never reads outside ``ex_items``."""
     _req(scores, "scores", torch.float32); _req(items, "items", torch.int32)
     if scores.shape != items.shape or scores.stride(0) != items.stride(0):
         raise ValueError("scores and items must have the same shape and row stride")
     if counts is not None:
         _req(counts, "counts", torch.int32)
     n = scores.shape[0]
+    ex_off = ex_items = None
+    ex_total = 0
+    if exclude is not None:
+        ex_off, ex_items = exclude
+        _req(ex_off, "exclude offsets", torch.int32); _req(ex_items, "exclude items", torch.int32)
+        if ex_off.shape != (n + 1,) or ex_items.dim() != 1:
+            raise ValueError(f"exclude must be (offsets [{n + 1}], items [E]) int32")
+        if ex_off.device != scores.device or ex_items.device != scores.device:
+            raise ValueError(f"exclude must be on {scores.device}")
+        ex_total = ex_items.numel()
+        if ex_total == 0:                  # a non-null pointer selects the filtering kernel; never read
+            ex_items = torch.zeros(1, dtype=torch.int32, device=scores.device)
     out_s = torch.empty((n, K), dtype=torch.float32, device=scores.device)
     out_i = torch.empty((n, K), dtype=torch.int32, device=scores.device)
     _check(lib().fps_row_topk(C.c_void_p(scores.data_ptr()), C.c_void_p(items.data_ptr()),
                               C.c_longlong(scores.stride(0)), int(n), int(scores.shape[1]),
                               C.c_void_p(counts.data_ptr() if counts is not None else None), int(K),
+                              C.c_void_p(ex_off.data_ptr() if ex_off is not None else None),
+                              C.c_void_p(ex_items.data_ptr() if ex_items is not None else None),
+                              int(ex_total),
                               C.c_void_p(out_s.data_ptr()), C.c_void_p(out_i.data_ptr()), _stream()),
            "row_topk")
     _bump()
