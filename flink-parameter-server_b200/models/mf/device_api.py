@@ -203,7 +203,9 @@ def ps_topk_generator_device(src, model, K: int = 100, workerK: int = 75, userMe
     table = the LEMP LENGTH bound) and the per-worker lists are merged.  ``model`` has the reference's
     orientation: ``Left((itemId, (len, vec)))`` / ``Right((userId, (len, vec)))``.  In a multi-rank job
     every rank passes its own part of the model and the *same* query stream.  Unknown users get an empty
-    list (the reference's ``invalidParam``).  Returns ``[(itemId, timestamp, [(score, itemId)])]``."""
+    list (the reference's ``invalidParam``).  Returns ``[(itemId, timestamp, [(score, itemId)])]``.
+    Vectors of up to 511 factors: the user table carries one extra "loaded" column and the scoring
+    kernel takes rows of at most 512 floats."""
     import numpy as np
     import torch.distributed as dist
 
@@ -300,7 +302,8 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
     Prequential at micro-batch granularity (``batch_size``; 1 reproduces the per-rating order).  The
     result is a pure function of the stream and the seed, whatever the number of ranks (init is Philox
     by id).  Rank 0 returns ``[(userId, itemId, timestamp, [(score, itemId)])]`` (other ranks ``[]``);
-    the model is in ``.users`` (the PS table) / ``.items`` (local partition)."""
+    the model is in ``.users`` (the PS table) / ``.items`` (local partition).  ``numFactors`` may be
+    up to 512 (the widest row of the scoring kernel)."""
     import torch.distributed as dist
 
     from ...store.sharded_table import ShardedTable

@@ -13,6 +13,8 @@ Algorithm (exact, tile-pruned -- the GPU-idiomatic replacement of the LEMP bucke
   select  top-K of the candidates.
 Scores are TF32 products accumulated in FP32; ``rescore=True`` recomputes the K winners in full
 FP32 (ordering among near-ties may then differ from the TF32 ranking by < 1e-3 relative).
+Rows may be up to ``native.TOPK_MAX_STRIDE`` = 512 floats wide; above 128 the scoring kernel streams
+the item table by 32-float K block (same passes, same exactness).
 
 Per-query exclusion (``topk(..., exclude=...)``, the seen-item filter of CollectTopKFromEachWorker):
 let ``E_q`` be the number of distinct excluded items of query ``q`` present in the table.  The
@@ -76,6 +78,7 @@ class DeviceTopK:
                  pass1_fraction: Optional[float] = None):
         if items.dim() != 2 or items.shape[1] % 4 != 0:
             raise ValueError("items must be [n_items, stride] with stride % 4 == 0")
+        native.check_topk_stride(items.shape[1])
         self.perm = self.inv_perm = None
         if sort_by_length:
             lens = items.norm(dim=1)

@@ -43,6 +43,8 @@ class DeviceSkipGram:
         self.rep_in = ReplicaCache(self.w_in, sync_every) if replica_cache else None
         self.rep_out = ReplicaCache(self.w_out, sync_every) if replica_cache else None
         self._ones = None
+        self._neighbours = None   # most_similar's scorer over the normalised W_in shard
+        self._snapshot_step = -1  # step_no the normalised snapshot was taken at
 
     def step(self, centers: torch.Tensor, contexts: torch.Tensor) -> None:
         if self._ones is None or self._ones.numel() != centers.numel():
@@ -69,6 +71,45 @@ class DeviceSkipGram:
         va, vb = self.w_in.pull(a), self.w_in.pull(b)
         return torch.nn.functional.cosine_similarity(va, vb)
 
+    def most_similar(self, words: torch.Tensor, K: int = 10):
+        """Cosine nearest neighbours of each query word among the input embeddings ``W_in``.
+
+        Returns ``(scores [n, K], word_ids [n, K])``, best first.  The query word itself is never in its
+        own list.  Rows with fewer than ``K`` other words end in ``(-3e38, -1)`` entries; a word whose
+        vector is zero gets cosine 0 for every neighbour.  Scores come from the TF32 tensor-core top-K
+        (``DistributedTopK``): they are within ~1e-3 of the fp32 cosine, and neighbours whose cosines
+        differ by less than that may be ordered differently from an fp32 ranking.
+
+        Every rank scores the queries against its own ``W_in`` shard, normalised row by row (a snapshot
+        kept until the next :meth:`step`); the queries are the raw rows, pulled by the scoring kernel.
+        Ranking by ``q . w / |w|`` is ranking by cosine, so only the K winners are divided by ``|q|``.
+        In a multi-rank job the call is collective: every rank passes the same ``words``."""
+        from .mf.device_topk import DistributedTopK
+
+        self.flush()
+        w = self.w_in
+        if w.world > 1:
+            w.barrier()                        # every rank's deltas are in the master shards
+        if self._snapshot_step != self.step_no:
+            ids = w.local_ids()
+            n_valid = max(int((ids < self.vocab).sum()), 1)     # slots past the vocabulary are padding
+            snap = torch.nn.functional.normalize(w.local[:n_valid], dim=1)  # zero rows stay zero
+            if self._neighbours is None:
+                self._neighbours = DistributedTopK(w, snap.contiguous(), ids[:n_valid], group=w.group)
+            else:                              # the scorer reads the snapshot in place
+                self._neighbours.local.items.copy_(snap)
+            self._snapshot_step = self.step_no
+        q = words.to(self.dev, torch.int64).reshape(-1).contiguous()
+        n = q.numel()
+        exclude = (torch.arange(n + 1, device=self.dev, dtype=torch.int64), q)   # each query's own id
+        sc, ids = self._neighbours.topk(q, K, exclude=exclude)
+        if sc.shape[1] < K:                    # a one-rank vocabulary smaller than K
+            sc = torch.nn.functional.pad(sc, (0, K - sc.shape[1]), value=-3.0e38)
+            ids = torch.nn.functional.pad(ids, (0, K - ids.shape[1]), value=-1)
+        qnorm = w.pull(q).norm(dim=1, keepdim=True)
+        cos = torch.where(qnorm > 0, sc / qnorm.clamp_min(1e-30), torch.zeros_like(sc))
+        return torch.where(ids >= 0, cos, sc), ids
+
     def score(self, centers: torch.Tensor, contexts: torch.Tensor) -> torch.Tensor:
         """sigmoid(W_in[center] . W_out[context]) -- the model's co-occurrence probability."""
         self.flush()
@@ -85,4 +126,7 @@ class DeviceSkipGram:
         self.w_in.barrier()
 
     def close(self):
+        gather = getattr(self._neighbours, "_p2p_gather", None)
+        if gather is not None:
+            gather.close()
         self.w_in.close(); self.w_out.close()

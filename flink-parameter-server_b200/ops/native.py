@@ -725,11 +725,22 @@ class TopkArgsC(C.Structure):
 
 
 TOPK_TILE = 128
+# widest row the scoring kernel takes: strides up to 128 floats keep whole item tiles in shared memory,
+# wider ones (up to 512) stream the items by 32-float K block (csrc/fps_topk_mma.cu)
+TOPK_MAX_STRIDE = 512
+
+
+def check_topk_stride(stride: int) -> None:
+    """Raise ``ValueError`` for rows wider than the top-K scoring kernel supports."""
+    if int(stride) > TOPK_MAX_STRIDE:
+        raise ValueError(f"device top-K supports rows of at most {TOPK_MAX_STRIDE} floats "
+                         f"(stride {int(stride)}); the kernel keeps the query block in shared memory")
 
 
 def topk_geometry(items: torch.Tensor, n_queries: int, tile_lo: int = 0, cand_cap: int = 0):
     """``(n_tiles, n_splits, seg_cap)`` the scoring kernel will use for this problem: every query row
     is handled by ``n_splits`` CTAs, each owning ``seg_cap = cand_cap // n_splits`` candidate slots."""
+    check_topk_stride(items.shape[1])
     a = TopkArgsC()
     a.n_queries = int(n_queries); a.n_items, a.stride = items.shape
     a.mode = -1; a.tile_lo = int(tile_lo); a.cand_cap = int(cand_cap)
@@ -747,7 +758,9 @@ def topk_mma(items: torch.Tensor, mode: int, *, q_ids: Optional[torch.Tensor] = 
     """wgmma scoring kernel (K6): queries (pulled from ``q_tab`` by id, or ``q_local``) x local
     ``items`` with a mode-dependent epilogue.  Only tiles ``tile_lo <= t < min(n_tiles, tile_limit[0])``
     are scored (``tile_limit``: optional int32 device scalar).  Mode 2 fills per-split candidate
-    segments: ``cand_count`` is ``[n_q, n_splits]`` (see :func:`topk_geometry`).  csrc/fps_topk_mma.cu."""
+    segments: ``cand_count`` is ``[n_q, n_splits]`` (see :func:`topk_geometry`).  Rows of up to
+    ``TOPK_MAX_STRIDE`` = 512 floats; wider ones raise ``ValueError``.  csrc/fps_topk_mma.cu."""
+    check_topk_stride(items.shape[1])
     _req(items, "items", torch.float32)
     n_items, stride = items.shape
     a = TopkArgsC()
