@@ -122,6 +122,7 @@ class DeviceOnlineMF:
         # buckets are ranges of rows of the table the fused kernel reads: the item shard (N = 1) or the
         # owner-major replica (row = owner * rows_per_shard + slot)
         table_rows = self.items.rows_per_shard * self.world if self.item_cache else self.num_items
+        self._table_rows = table_rows
         while -(-table_rows >> self.block_shift) > native.BUCKET_MAX:
             self.block_shift += 1
         self.block_buckets = max(1, -(-table_rows >> self.block_shift))
@@ -153,7 +154,12 @@ class DeviceOnlineMF:
         fed = False
         ring = self.output_ring
         out_args = ring.kernel_args() if ring is not None else None
-        if self.item_blocking and self.block_buckets > 1:
+        # The deal pays only when rows are revisited inside the launch: a local-table micro-batch with no more
+        # records than the table has rows touches a row about once whatever the order (on one H100 the fused
+        # kernel took the same time with and without it, profiles/h100_mf_step_breakdown.json).  The replica
+        # mode always deals: the bucket histogram feeds its flush policy.
+        revisits = self.item_cache or n_records * (1 + neg) > self._table_rows
+        if self.item_blocking and self.block_buckets > 1 and revisits:
             hashed = self.item_cache and self.items.mode == native.PART_HASH
             fed = hashed
             users, items, ratings = native.bucket_by_item(

@@ -10,15 +10,17 @@
 // SGD has no ordering contract inside a micro-batch (the reference's workers interleave arbitrarily),
 // so the reordering is semantically free.
 //
-// Two streaming kernels, no host synchronisation: a histogram over the bucket ids, then a scatter in
-// which each CTA reserves one contiguous run per bucket (shared-memory ranks + one global atomic per
-// (CTA, bucket)).  Cost: read the batch twice, write it once (~100 MB for 4M packed records).
+// One cooperative kernel, no host synchronisation (fps_bucket_deal_kernel below): a histogram over the bucket
+// ids, a grid sync, then a scatter in which each CTA reserves one contiguous run per bucket (shared-memory ranks
+// + one global atomic per (CTA, bucket)).  Cost: read the batch from HBM once and from L2 once, write it once.
 #include <cuda_fp16.h>
+#include <cooperative_groups.h>
 #include "fps_common.cuh"
+
+namespace cg = cooperative_groups;
 
 #define BK_MAX 64        // max buckets
 #define BK_THREADS 256
-#define BK_PER_THREAD 8  // records per thread in the scatter kernel
 
 struct BucketArgs {
   const void* users;   // format 0: ids; format 1: packed64 records (user:26 | item:22 | fp16 rating)
@@ -29,7 +31,7 @@ struct BucketArgs {
   int id_bytes;        // 4 or 8 (format 0)
   int shift;           // bucket = row >> shift, row = owner(item) * rps + slot(item): the row index of the
   int n_buckets;       //   owner-major table the fused kernel reads (num_shards == 1: row == item)
-  unsigned int* scratch;  // [2 * BK_MAX]: totals, cursors (zeroed by the launcher)
+  unsigned int* scratch;  // [2 * BK_MAX]: totals, cursors (zeroed by the kernel)
   void* out_users;
   void* out_items;
   float* out_ratings;
@@ -61,56 +63,48 @@ __device__ __forceinline__ int bk_bucket(const BucketArgs& a, long long item) {
   return (int)(b < a.n_buckets ? b : a.n_buckets - 1);
 }
 
-__global__ void __launch_bounds__(BK_THREADS) fps_bucket_hist_kernel(const BucketArgs a) {
+// One cooperative launch per micro-batch.  Each CTA owns a contiguous chunk of the batch:
+//   1. CTA 0 zeroes the counters while every CTA counts its chunk's buckets in shared memory;  grid sync;
+//   2. the CTA counts go to the global totals (and the per-destination feed);  grid sync;
+//   3. each CTA reserves one run per bucket (exclusive prefix of the totals + a cursor atomic) and re-reads its
+//      chunk -- an L2 hit: the batch is a few MB -- to write every record at its run's next slot.
+// Against a memset + histogram kernel + scatter kernel this reads the batch from HBM once and leaves two
+// stream operations (and the launch gaps around them) out of every micro-batch.
+__global__ void __launch_bounds__(BK_THREADS) fps_bucket_deal_kernel(const BucketArgs a, long long per_cta) {
   __shared__ unsigned int hist[BK_MAX];
+  __shared__ unsigned int base[BK_MAX];
   __shared__ unsigned int ohist[FPS_MAX_SHARDS];
+  cg::grid_group grid = cg::this_grid();
   if (threadIdx.x < BK_MAX) hist[threadIdx.x] = 0;
   if (threadIdx.x < FPS_MAX_SHARDS) ohist[threadIdx.x] = 0;
+  if (blockIdx.x == 0 && threadIdx.x < 2 * BK_MAX) a.scratch[threadIdx.x] = 0;
   __syncthreads();
   const bool feed = a.pending != nullptr;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < a.n;
-       i += (long long)gridDim.x * blockDim.x) {
+  const long long lo = (long long)blockIdx.x * per_cta;
+  const long long hi = lo + per_cta < a.n ? lo + per_cta : a.n;
+  for (long long i = lo + threadIdx.x; i < hi; i += BK_THREADS) {
     const long long item = bk_item(a, i);
     atomicAdd(&hist[bk_bucket(a, item)], 1u);
     if (feed) atomicAdd(&ohist[bk_owner(a, item)], 1u);
   }
   __syncthreads();
+  grid.sync();
   if (threadIdx.x < a.n_buckets && hist[threadIdx.x] != 0)
     atomicAdd(a.scratch + threadIdx.x, hist[threadIdx.x]);
   if (feed && threadIdx.x < a.num_shards && ohist[threadIdx.x] != 0)
     atomicAdd(a.pending + threadIdx.x, (unsigned long long)ohist[threadIdx.x]);
-}
-
-__global__ void __launch_bounds__(BK_THREADS) fps_bucket_scatter_kernel(const BucketArgs a) {
-  __shared__ unsigned int hist[BK_MAX];
-  __shared__ unsigned int base[BK_MAX];
-  if (threadIdx.x < BK_MAX) hist[threadIdx.x] = 0;
-  __syncthreads();
-  const long long chunk0 = (long long)blockIdx.x * (BK_THREADS * BK_PER_THREAD);
-  int bucket[BK_PER_THREAD];
-  unsigned int rank[BK_PER_THREAD];
-#pragma unroll
-  for (int u = 0; u < BK_PER_THREAD; ++u) {
-    const long long i = chunk0 + u * BK_THREADS + threadIdx.x;
-    bucket[u] = -1;
-    if (i < a.n) {
-      bucket[u] = bk_bucket(a, bk_item(a, i));
-      rank[u] = atomicAdd(&hist[bucket[u]], 1u);
-    }
-  }
-  __syncthreads();
+  grid.sync();
   if (threadIdx.x < a.n_buckets) {
     unsigned int start = 0;  // exclusive prefix of the bucket totals
     for (int b = 0; b < threadIdx.x; ++b) start += a.scratch[b];
     const unsigned int mine = hist[threadIdx.x];
     base[threadIdx.x] = start + (mine ? atomicAdd(a.scratch + BK_MAX + threadIdx.x, mine) : 0u);
+    hist[threadIdx.x] = 0;   // from here on: the next free slot of this CTA's run
   }
   __syncthreads();
-#pragma unroll
-  for (int u = 0; u < BK_PER_THREAD; ++u) {
-    if (bucket[u] < 0) continue;
-    const long long i = chunk0 + u * BK_THREADS + threadIdx.x;
-    const long long o = (long long)base[bucket[u]] + rank[u];
+  for (long long i = lo + threadIdx.x; i < hi; i += BK_THREADS) {
+    const int b = bk_bucket(a, bk_item(a, i));
+    const long long o = (long long)base[b] + atomicAdd(&hist[b], 1u);
     if (a.format == 1) {
       reinterpret_cast<unsigned long long*>(a.out_users)[o] =
           reinterpret_cast<const unsigned long long*>(a.users)[i];
@@ -130,12 +124,18 @@ __global__ void __launch_bounds__(BK_THREADS) fps_bucket_scatter_kernel(const Bu
 extern "C" int fps_bucket_by_item(const BucketArgs* a, int num_sms, cudaStream_t stream) {
   if (a->n <= 0) return 0;
   if (a->n_buckets < 1 || a->n_buckets > BK_MAX || a->n >= (1ll << 32)) return -1301;
-  cudaError_t e = cudaMemsetAsync(a->scratch, 0, 2 * BK_MAX * sizeof(unsigned int), stream);
+  int occ = 0;
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fps_bucket_deal_kernel, BK_THREADS, 0);
   if (e != cudaSuccess) return (int)e;
-  long long hb = (a->n + BK_THREADS - 1) / BK_THREADS;
-  if (hb > (long long)num_sms * 8) hb = (long long)num_sms * 8;
-  fps_bucket_hist_kernel<<<(int)hb, BK_THREADS, 0, stream>>>(*a);
-  const long long per = BK_THREADS * BK_PER_THREAD;
-  fps_bucket_scatter_kernel<<<(int)((a->n + per - 1) / per), BK_THREADS, 0, stream>>>(*a);
+  long long grid = (long long)num_sms * (occ < 4 ? occ : 4);   // every CTA must be resident (grid sync)
+  const long long need = (a->n + BK_THREADS - 1) / BK_THREADS;
+  if (grid > need) grid = need;
+  if (grid < 1) grid = 1;
+  long long per_cta = (a->n + grid - 1) / grid;
+  BucketArgs args = *a;
+  void* params[] = {&args, &per_cta};
+  e = cudaLaunchCooperativeKernel((const void*)fps_bucket_deal_kernel, dim3((unsigned)grid), dim3(BK_THREADS),
+                                  params, 0, stream);
+  if (e != cudaSuccess) return (int)e;
   return (int)cudaGetLastError();
 }

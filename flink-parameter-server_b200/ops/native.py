@@ -416,8 +416,8 @@ BUCKET_MAX = 64
 def bucket_by_item(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Optional[torch.Tensor],
                    shift: int, n_buckets: int, scratch: torch.Tensor, num_shards: int = 1,
                    rows_per_shard: int = 0, pending: Optional[torch.Tensor] = None):
-    """Reorder a micro-batch by ``row(item) >> shift`` (L2 blocking of the item table,
-    csrc/fps_bucket.cu); ``row`` is the row of the owner-major table the fused kernel reads
+    """Reorder a micro-batch by ``row(item) >> shift`` (L2 blocking of the item table, one cooperative
+    kernel in csrc/fps_bucket.cu); ``row`` is the row of the owner-major table the fused kernel reads
     (``(item % num_shards) * rows_per_shard + item // num_shards``; plain ``item`` for one shard).
     ``items=None``: ``users`` holds packed64 records.  ``scratch``: int32 device tensor of
     ``2 * BUCKET_MAX`` elements.  ``pending``: optional int64 ``[num_shards]`` device counters that
@@ -447,7 +447,7 @@ def bucket_by_item(users: torch.Tensor, items: Optional[torch.Tensor], ratings: 
         _req(pending, "pending", torch.int64)
         a.pending = pending.data_ptr()
     _check(lib().fps_bucket_by_item(C.byref(a), sm_count(users.device.index), _stream()), "bucket_by_item")
-    _bump(2)
+    _bump()
     return ou, oi, orat
 
 
