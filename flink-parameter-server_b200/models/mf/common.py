@@ -185,6 +185,27 @@ class SGDUpdater(FactorUpdater):
         return self.lr * e * item, self.lr * e * user
 
 
+def bpr_delta(u: Vector, vi: Vector, vj: Vector, lr: float, reg: float):
+    """One BPR step (Rendle et al. 2009) on the triple ``(u, i, j)``: the SGD deltas of
+    ``softplus(-x) + reg/2 * (|u|^2 + |vi|^2 + |vj|^2)`` with ``x = u . (vi - vj)``, all computed from the
+    given values, and the triple's loss ``softplus(-x)``.  Returns ``(du, dvi, dvj, loss)``; the
+    reference of the device kernel ``fps_mf_bpr``."""
+    x = float(np.dot(u, vi - vj))
+    g = lr * _sigmoid(-x)
+    du = g * (vi - vj) - lr * reg * u
+    dvi = g * u - lr * reg * vi
+    dvj = -g * u - lr * reg * vj
+    loss = max(-x, 0.0) + math.log1p(math.exp(-abs(x)))
+    return du, dvi, dvj, loss
+
+
+def require_pointwise(backend: str, kw: dict) -> None:
+    """The host tiers (``backend="local"`` / ``"native"``) train the pointwise loss only."""
+    if backend != "device" and (kw.get("loss", "pointwise") != "pointwise" or kw.get("regularization", 0)):
+        raise ValueError(f"loss={kw.get('loss')!r} / regularization need backend='device' "
+                         f"(backend={backend!r} trains the pointwise loss only)")
+
+
 # ---- top-K ------------------------------------------------------------------------------
 class TopKQueue:
     """Bounded min-heap of ``(score, itemId)`` keeping the K largest (Utils.scala:13-18)."""

@@ -46,7 +46,23 @@ class DeviceOnlineMF:
                  sync_interval_ms: Optional[float] = None, item_blocking: Optional[bool] = None,
                  block_bytes: int = 16 << 20, flush_count: Optional[int] = None,
                  flush_require: str = "any", replica_own_inplace: Optional[bool] = None,
-                 output_ring=None):
+                 output_ring=None, loss: str = "pointwise", regularization: float = 0.0):
+        """``loss="bpr"``: pairwise (Bayesian Personalised Ranking) updates, each positive rating paired
+        with ``negative_sample_rate`` negatives (sampled) or with the ``negatives=`` of :meth:`step`;
+        ``regularization`` is its L2 weight.  The pointwise loss has no regulariser."""
+        if loss not in ("pointwise", "bpr"):
+            raise ValueError(f"loss must be 'pointwise' or 'bpr', got {loss!r}")
+        self.loss, self.reg = loss, float(regularization)
+        if loss == "pointwise" and self.reg != 0.0:
+            raise ValueError("regularization is only supported with loss='bpr'")
+        if loss == "bpr":
+            if output_ring is not None:
+                raise ValueError("the per-update output ring is not supported with loss='bpr'")
+            if kernel == "tma":
+                raise ValueError("kernel='tma' is not supported with loss='bpr'")
+            if item_blocking:
+                raise ValueError("item_blocking is not supported with loss='bpr'")
+            item_blocking = False
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.cuda_device = torch.device("cuda", self.device)
         self.group = group
@@ -64,8 +80,10 @@ class DeviceOnlineMF:
         # pull limiter (WL:196-250) = device credit counter [credits, stalls] consumed inside the fused kernel
         # (a warp takes its credits all at once, so limits below one warp's worth of pulls fall back to the
         # static form of the limiter: a capped grid)
+        # (the BPR kernel has only the static form)
         self.credits = (torch.tensor([self.pull_limit, 0], dtype=torch.int32, device=self.cuda_device)
-                        if self.pull_limit >= 32 and os.environ.get("FPS_STATIC_LIMITER", "0") != "1" else None)
+                        if self.pull_limit >= 32 and os.environ.get("FPS_STATIC_LIMITER", "0") != "1"
+                        and loss == "pointwise" else None)
         self.output_ring = output_ring     # E5: per-update (user, vector) output stream (runtime/output_ring.py)
         with torch.cuda.device(self.device):
             # parameter server: item vectors, sharded item % psParallelism
@@ -79,7 +97,8 @@ class DeviceOnlineMF:
                                      device=self.cuda_device)
             native.init_rows(self.users, self.k, self.rank, self.world, native.PART_HASH, n_local,
                              seed * 2 + 2, range_min, range_max)
-            self.stats = torch.zeros(2, dtype=torch.float32, device=self.cuda_device)
+            # pointwise: [sum (r - u.v)^2, updates]; BPR: [sum softplus(-x), triples, triples with x > 0]
+            self.stats = torch.zeros(3 if loss == "bpr" else 2, dtype=torch.float32, device=self.cuda_device)
             self.nan_flag = torch.zeros(1, dtype=torch.int32, device=self.cuda_device)
             # K5: per-user memory of recently seen items (userMemory of the reference, default 128
             # there; 0 here = sample uniformly inside the fused kernel, rejecting only the positive)
@@ -139,9 +158,15 @@ class DeviceOnlineMF:
             self.replica.flush()
 
     def step(self, users: torch.Tensor, items: Optional[torch.Tensor] = None,
-             ratings: Optional[torch.Tensor] = None) -> None:
+             ratings: Optional[torch.Tensor] = None, negatives: Optional[torch.Tensor] = None) -> None:
         """Process one micro-batch of ratings whose users belong to this worker (async SGD).
-        ``step(packed)`` with a single int64 tensor takes packed64 records (``native.pack_ratings``)."""
+        ``step(packed)`` with a single int64 tensor takes packed64 records (``native.pack_ratings``).
+        ``negatives`` (``loss="bpr"`` only): ``[n, m]`` item ids paired with each rating, ``-1`` = none."""
+        if self.loss == "bpr":
+            self._step_bpr(users, items, ratings, negatives)
+            return
+        if negatives is not None:
+            raise ValueError("negatives= needs loss='bpr'")
         neg = self.neg
         if self.user_memory > 0:
             # negatives drawn by the sampler kernel against the per-user seen ring; the fused kernel
@@ -189,6 +214,40 @@ class DeviceOnlineMF:
         self.step_no += 1
         METRICS.inc("mf_ratings", users.numel())
 
+    def _step_bpr(self, users, items, ratings, negatives) -> None:
+        if negatives is not None:
+            if self.item_cache:
+                raise ValueError("negatives= is not supported in the replica (item_cache) mode")
+            n = int(negatives.shape[1]) if negatives.dim() == 2 else 0
+        elif self.neg < 1:
+            raise ValueError("loss='bpr' needs negative_sample_rate >= 1 or explicit negatives=")
+        elif self.user_memory > 0:
+            # negatives that avoid the user's recent items: the sampler's expanded [n, 1 + m] records,
+            # with the negatives it could not find voided
+            per = 1 + self.neg
+            ou, oi, orat = native.neg_sample(users, items, ratings, self.neg, self.num_items, self.seen,
+                                             self.seen_pos, self.world, seed=self.seed, step=self.step_no)
+            ou, oi = ou.view(-1, per), oi.view(-1, per)
+            negatives = torch.where(ou[:, 1:] >= 0, oi[:, 1:], torch.full_like(oi[:, 1:], -1)).contiguous()
+            users, items, ratings = ou[:, 0].contiguous(), oi[:, 0].contiguous(), orat.view(-1, per)[:, 0].contiguous()
+            n = self.neg
+        else:
+            n = self.neg                   # drawn inside the kernel
+        if self.output_ring is not None:
+            raise ValueError("the per-update output ring is not supported with loss='bpr'")
+        n_pos = users.numel()
+        cand, reserve = self.items.table_c, 0
+        if self.item_cache:
+            # uniform per-destination counts feed the flush policy (BPR batches are not dealt into buckets)
+            self.replica.after_step(n_pos * n, fed=False)
+            cand, reserve = self.replica.table_c, self.replica.reserve_total()
+        native.mf_bpr_fused(users, items, ratings, self.users, cand, self.lr, self.reg, negatives=negatives,
+                            n_neg=n, num_items=self.num_items, seed=self.seed, step=self.step_no,
+                            anchor_div=self.world, stats=self.stats, nan_flag=self.nan_flag,
+                            max_inflight_rows=self.pull_limit, reserve_total=reserve)
+        self.step_no += 1
+        METRICS.inc("mf_ratings", n_pos)
+
     def make_graph_step(self, batch_size: int, packed: bool = True):
         """CUDA-graph a fixed-size micro-batch step for launch-bound streaming (small batches).
 
@@ -220,11 +279,12 @@ class DeviceOnlineMF:
 
         Yields one host-side ``(sum_sq_err, n_updates)`` per micro-batch (device -> host read of
         the step's result), lagging the launch by one step so copies, kernels and reads overlap.
+        With ``loss="bpr"`` the pair is ``(sum softplus(-x), n_triples)``.
         """
         pf = DevicePrefetcher(host_batches, self.cuda_device, depth=2)
         self.prefetcher = pf
         pending = []
-        ring = [torch.empty(2, dtype=torch.float32).pin_memory() for _ in range(4)]
+        ring = [torch.empty(self.stats.numel(), dtype=torch.float32).pin_memory() for _ in range(4)]
         i = 0
         for batch in pf:
             self.stats.zero_()

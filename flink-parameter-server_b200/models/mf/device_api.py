@@ -72,10 +72,16 @@ def ps_online_mf_device(src, numFactors=10, rangeMin=-0.01, rangeMax=0.01, learn
                         numUsers: Optional[int] = None, numItems: Optional[int] = None,
                         batch_size: int = 1 << 16, group=None, epochs: int = 1,
                         userMemory: int = 128, updateOutput: Optional[int] = None,
-                        outputFlushCount: int = 1, outputFlushMs: Optional[float] = None) -> ResultStream:
+                        outputFlushCount: int = 1, outputFlushMs: Optional[float] = None,
+                        loss: str = "pointwise", regularization: float = 0.0) -> ResultStream:
     """``updateOutput=n``: also emit ``Left((userId, userVector))`` for one update in ``n`` (``1`` = every
     update, the reference's worker output PSOnlineMatrixFactorizationWorker.scala:52) through the device
-    output ring (count / timer flushed on the device); the final dump then holds only the item shard."""
+    output ring (count / timer flushed on the device); the final dump then holds only the item shard.
+    ``loss="bpr"``: pairwise updates, every rating > 0 paired with ``negativeSampleRate`` sampled
+    negatives, L2 weight ``regularization`` (see :class:`DeviceOnlineMF`); it has no per-update output,
+    so ``updateOutput`` with ``loss="bpr"`` raises ``ValueError``."""
+    if updateOutput and loss != "pointwise":
+        raise ValueError("updateOutput (the per-update output ring) is not supported with loss='bpr'")
     recs = None
     if numUsers is None or numItems is None:
         recs = list(src.collect() if hasattr(src, "collect") else src)
@@ -90,7 +96,8 @@ def ps_online_mf_device(src, numFactors=10, rangeMin=-0.01, rangeMax=0.01, learn
                            negativeSampleRate, pull_limit=int(pullLimit or 0),
                            group=group, seed=seed, err_mode=ERR_PLAIN if plain_residual else ERR_SIGMOID,
                            track_touched=True,
-                           user_memory=min(int(userMemory), 256) if negativeSampleRate > 0 else 0)
+                           user_memory=min(int(userMemory), 256) if negativeSampleRate > 0 else 0,
+                           loss=loss, regularization=regularization)
     ring, updates = None, []
     if updateOutput:
         from ...runtime.output_ring import OutputRing
@@ -281,7 +288,8 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
                                            learningRate=0.01, negativeSampleRate=0, userMemory=65535,
                                            K=100, workerK=None, pullLimit=0, seed=0, plain_residual=False,
                                            numUsers: Optional[int] = None, numItems: Optional[int] = None,
-                                           batch_size: int = 4096, group=None):
+                                           batch_size: int = 4096, group=None, loss: str = "pointwise",
+                                           regularization: float = 0.0):
     """Online MF plus a top-K list for every incoming rating, computed BEFORE the model sees that rating
     (prequential evaluation; ``psOnlineLearnerAndGenerator``,
     PSOnlineMatrixFactorizationAndTopKGenerator.scala:51-101) on the device tier, any number of ranks.
@@ -309,6 +317,12 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
     from ...store.sharded_table import ShardedTable
     from .device_topk import DeviceTopK, DistributedTopK
 
+    if loss not in ("pointwise", "bpr"):
+        raise ValueError(f"loss must be 'pointwise' or 'bpr', got {loss!r}")
+    if loss == "pointwise" and regularization != 0:
+        raise ValueError("regularization is only supported with loss='bpr'")
+    if loss == "bpr" and negativeSampleRate < 1:
+        raise ValueError("loss='bpr' needs negativeSampleRate >= 1")
     recs = list(src.collect() if hasattr(src, "collect") else src)
     if numUsers is None:
         numUsers = 1 + max((r.user for r in recs), default=0)
@@ -326,7 +340,7 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
     native.init_rows(items, numFactors, rank, world, native.PART_HASH, n_local, seed * 2 + 1, rangeMin, rangeMax)
     local_ids = torch.arange(n_local, device=dev, dtype=torch.int64) * world + rank
     n_valid = int((local_ids < numItems).sum())
-    stats = torch.zeros(2, dtype=torch.float32, device=dev)
+    stats = torch.zeros(3 if loss == "bpr" else 2, dtype=torch.float32, device=dev)
     nan_flag = torch.zeros(1, dtype=torch.int32, device=dev)
     err_mode = ERR_PLAIN if plain_residual else ERR_SIGMOID
     wk = max(workerK or K, K)
@@ -363,12 +377,20 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
             clash = neg_item == i[:, None]
             neg_item = torch.where(clash, ((neg_slot + 1) % n_valid * world + rank).to(torch.int32), neg_item)
             neg_item = torch.where(mine[:, None], neg_item, torch.full_like(neg_item, -1))
-            ti = torch.cat([ti, neg_item.reshape(-1)])
-            tu = torch.cat([u, u[:, None].expand(-1, negativeSampleRate).reshape(-1)])
-            tr = torch.cat([rt, torch.zeros(neg_item.numel(), device=dev)])
-        native.mf_sgd_fused(ti.contiguous(), tu.contiguous(), tr.contiguous(), items, world, users.table_c,
-                            learningRate, err_mode=err_mode, stats=stats, nan_flag=nan_flag,
-                            max_inflight_rows=int(pullLimit or 0), kernel="reg")
+            if loss == "pointwise":
+                ti = torch.cat([ti, neg_item.reshape(-1)])
+                tu = torch.cat([u, u[:, None].expand(-1, negativeSampleRate).reshape(-1)])
+                tr = torch.cat([rt, torch.zeros(neg_item.numel(), device=dev)])
+        if loss == "bpr":
+            if n_valid > 0:
+                # anchors = users on the PS, candidates = this rank's item rows (slot = item // world)
+                native.mf_bpr_fused(u, ti, rt, users.table_c, items, learningRate, regularization,
+                                    negatives=neg_item.contiguous(), cand_div=world, stats=stats,
+                                    nan_flag=nan_flag, max_inflight_rows=int(pullLimit or 0))
+        else:
+            native.mf_sgd_fused(ti.contiguous(), tu.contiguous(), tr.contiguous(), items, world, users.table_c,
+                                learningRate, err_mode=err_mode, stats=stats, nan_flag=nan_flag,
+                                max_inflight_rows=int(pullLimit or 0), kernel="reg")
         users.barrier()                      # pushes of this micro-batch are in the PS before the next pulls
     if int(nan_flag.item()) != 0:
         from ...errors import FactorIsNotANumberException

@@ -20,7 +20,7 @@ from ...limiter import addPullLimiter
 from ...runtime.stream import as_stream
 from ...runtime.transform import transform
 from ...utils.eof import EOF, with_eof
-from .common import Rating, RangedRandomFactorInitializerDescriptor, SGDUpdater, vectorSum
+from .common import Rating, RangedRandomFactorInitializerDescriptor, SGDUpdater, require_pointwise, vectorSum
 from .online import NegativeSampler
 
 
@@ -103,6 +103,7 @@ def psOfflineMF(src, numFactors: int = 10, rangeMin: float = -0.01, rangeMax: fl
                 plain_residual: bool = False, shuffle: bool = False, backend: str = "local",
                 **device_kw):
     hostPullLimit = 1600 if pullLimit is None else pullLimit   # reference default (JVM queue bound)
+    require_pointwise(backend, device_kw)
     if backend == "native":
         from .native_api import ps_mf_native
 

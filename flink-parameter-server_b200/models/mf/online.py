@@ -26,7 +26,7 @@ from ...limiter import addPullLimiter
 from ...runtime.stream import DataStream, ResultStream, as_stream
 from ...runtime.transform import transform
 from ...server.logics import SimplePSLogic
-from .common import (Rating, RangedRandomFactorInitializerDescriptor, SGDUpdater, vectorSum)
+from .common import (Rating, RangedRandomFactorInitializerDescriptor, SGDUpdater, require_pointwise, vectorSum)
 
 
 class NegativeSampler:
@@ -125,6 +125,7 @@ def psOnlineMF(src, numFactors: int = 10, rangeMin: float = -0.01, rangeMax: flo
     ``backend="local"``: arbitrary-logic Python engine; ``"native"``: the same protocol on the C++ host
     engine (threads + SPSC rings, ``ops/csrc/fps_host.cpp``); ``"device"``: fused GPU kernels."""
     hostPullLimit = 1600 if pullLimit is None else pullLimit   # reference default (JVM queue bound)
+    require_pointwise(backend, device_kw)
     if backend == "native":
         from .native_api import ps_mf_native
 

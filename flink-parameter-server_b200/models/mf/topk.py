@@ -28,7 +28,7 @@ from ...parallel.partitioner import stable_hash
 from ...runtime.stream import DataStream, as_stream
 from ...runtime.transform import transform, transformWithDoubleModelLoad
 from ...server.logics import SimplePSLogic
-from .common import (IDGenerator, Partitioner, RangedRandomFactorInitializerDescriptor, Rating,
+from .common import (IDGenerator, Partitioner, RangedRandomFactorInitializerDescriptor, Rating, require_pointwise,
                      RichRating, SGDUpdater, TopKQueue, attachLength, vectorSum)
 from .pruning import (COORD, INCR, LC, LENGTH, LI, LEMPPruningStrategy, coordPruning, focus_coordinate,
                       focus_set, incrPruning, lengthPruning)
@@ -279,6 +279,7 @@ def psOnlineLearnerAndGenerator(src, numFactors: int = 10, rangeMin: float = -0.
     """Returns ``[(userId, itemId, timestamp, [(score, itemId)])]`` -- one top-K per rating, computed
     BEFORE the model is updated with that rating (prequential evaluation).  ``backend="device"``:
     ``models/mf/device_api.py::ps_online_learner_and_generator_device``."""
+    require_pointwise(backend, device_kw)
     if backend == "device":
         from .device_api import ps_online_learner_and_generator_device
 

@@ -1,0 +1,249 @@
+// Pairwise (BPR, Rendle et al. 2009) matrix-factorisation step for sm_90a: pull + SGD + push of one
+// (anchor, positive, negative) triple in one kernel, next to the pointwise step of fps_core.cu.
+//
+// For every positive record (a, i) with rating > 0 and each of its n negatives j:
+//   x   = u . (v_i - v_j)                       (u = anchor row, v = candidate rows, all as pulled)
+//   g   = lr * sigmoid(-x)
+//   u   += g * (v_i - v_j) - lr*reg*u           (REDG.ADD.F32x4)
+//   v_i += g * u           - lr*reg*v_i         (push)
+//   v_j += -g * u          - lr*reg*v_j         (push)
+//   stats[0] += softplus(-x), stats[1] += 1, stats[2] += (x > 0)
+// One lane-group handles one positive: u and v_i are pulled once, the n negatives are pulled in turn,
+// and the summed u / v_i deltas of the n triples are pushed once.  Every delta is computed from the
+// values as pulled (the contract of the fused pointwise kernel), so a batch whose anchors and
+// candidates are all distinct gives the same result in any schedule.
+//
+// Negatives come from an int tensor [n_pos, n] (-1 voids a triple) or are drawn in the kernel from
+// the K5 Philox stream of fps_mf_sgd_fused_kernel (key (pos, j, step, seed), uniform over
+// [0, num_items), the positive rejected by a shift of 1 + s.z % 7).  The shift is reduced modulo
+// num_items - 1 so that it never lands back on the positive: identical to K5 for num_items >= 8.
+//
+// Rows: the anchor rows and the candidate rows are each read either from a worker-local table
+// (slot = id / div) or through a ShardTable (local shard, NVLink peer shard, or a replica); the
+// candidate deltas may go to a separate push table (replica staging).  The pointwise learner keeps
+// users on the PS and items local, the MF model the other way round; both use this one kernel.
+#include <cuda_fp16.h>
+#include "fps_common.cuh"
+
+struct BprArgs {
+  const void* users;          // anchor ids, or packed64 records (user:26 | item:22 | rating fp16:16)
+  const void* items;          // positive candidate ids
+  const float* ratings;       // records with rating <= 0 are skipped
+  const void* negatives;      // [n_pos, n_neg] candidate ids, -1 = void; nullptr = sampled in the kernel
+  long long n_pos;
+  int n_neg;
+  int format;                 // 0: users/items/ratings arrays; 1: packed64 records in `users`
+  long long num_items;        // sampled negatives: id range [0, num_items)
+  unsigned long long seed;    // sampled negatives: stream key
+  unsigned long long step;    // sampled negatives: stream counter (micro-batch number)
+  float lr;
+  float reg;
+  float* anchor_table;        // worker-local [rows, stride] when anchor_sharded == 0
+  int anchor_div;             //   slot = id / anchor_div
+  int anchor_shift;           //   log2(anchor_div) if a power of two, else -1
+  int anchor_sharded;         // != 0: anchor rows are read and pushed through anchor_tab
+  int cand_sharded;           // != 0: candidate rows are read through cand_tab
+  ShardTable anchor_tab;
+  float* cand_table;          // worker-local [rows, stride] when cand_sharded == 0
+  int cand_div;
+  int cand_shift;
+  ShardTable cand_tab;
+  int use_push_tab;           // != 0 (with cand_sharded): candidate deltas go to push_tab
+  int stride;                 // row stride in floats, shared by every table
+  ShardTable push_tab;
+  float* stats;               // [0] += softplus(-x), [1] += #triples, [2] += #(x > 0)
+  int* nan_flag;              // set to 1 if a non-finite update was produced
+  int reserve_total;          // CTA slots left free on the whole GPU (the replica exchange CTAs)
+  int pad_;
+};
+
+template <typename IdT>
+__device__ __forceinline__ float* bpr_row(float* local, int div, int shift, int sharded,
+                                          const ShardTable& t, IdT id, int stride) {
+  if (sharded) return fps_row_t<IdT>(t, id);
+  return local + fps_user_slot<IdT>(id, div, shift) * (size_t)stride;
+}
+
+__device__ __forceinline__ float4 bpr_axpy(float a, float4 x, float b, float4 y) {
+  return make_float4(a * x.x + b * y.x, a * x.y + b * y.y, a * x.z + b * y.z, a * x.w + b * y.w);
+}
+
+template <typename IdT, int LPR, int VPL, int MINB, int FMT>
+__global__ void __launch_bounds__(256, MINB) fps_mf_bpr_kernel(const __grid_constant__ BprArgs a) {
+  const int lane = threadIdx.x & (LPR - 1);
+  const long long group = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LPR;
+  const long long n_groups = ((long long)gridDim.x * blockDim.x) / LPR;
+  const int stride = a.stride;
+  const int nvec = stride >> 2;
+  const float decay = a.lr * a.reg;
+  const IdT* __restrict__ negs = reinterpret_cast<const IdT*>(a.negatives);
+  float loss_acc = 0.f, cnt_acc = 0.f, ok_acc = 0.f;
+  bool bad = false;
+
+  // the trip count is the same for every lane of a warp (n_groups is a multiple of 32 / LPR), so the
+  // full-warp shuffles of fps_group_sum below always see the whole warp
+  const long long n_round = ((a.n_pos + n_groups - 1) / n_groups) * n_groups;
+  for (long long pos = group; pos < n_round; pos += n_groups) {
+    bool ok = pos < a.n_pos;
+    IdT anchor = 0, item = 0;
+    if (ok) {
+      float rating;
+      if (FMT == 1) {
+        const unsigned long long rec = reinterpret_cast<const unsigned long long*>(a.users)[pos];
+        anchor = (IdT)(rec >> 38);
+        item = (IdT)((rec >> 16) & 0x3FFFFFull);
+        rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
+      } else {
+        anchor = reinterpret_cast<const IdT*>(a.users)[pos];
+        item = reinterpret_cast<const IdT*>(a.items)[pos];
+        rating = a.ratings[pos];
+      }
+      // rating <= 0 (a pointwise stream's explicit negatives) and voided records are not positives
+      ok = rating > 0.f && anchor >= 0 && item >= 0;
+    }
+    float* up = bpr_row<IdT>(a.anchor_table, a.anchor_div, a.anchor_shift, a.anchor_sharded,
+                             a.anchor_tab, anchor, stride);
+    float* vip = bpr_row<IdT>(a.cand_table, a.cand_div, a.cand_shift, a.cand_sharded, a.cand_tab,
+                              item, stride);
+    float4 u[VPL], vi[VPL], du[VPL];
+#pragma unroll
+    for (int c = 0; c < VPL; ++c) {
+      const int q = lane + c * LPR;
+      if (ok && q < nvec) {
+        u[c] = a.anchor_sharded ? fps_ld_row4(up + 4 * q) : *reinterpret_cast<const float4*>(up + 4 * q);
+        vi[c] = fps_ld_row4(vip + 4 * q);   // the PULLs
+      } else {
+        u[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+        vi[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      du[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    float g_sum = 0.f;
+    int n_live = 0;
+    for (int j = 0; j < a.n_neg; ++j) {
+      long long neg = -1;
+      if (ok) {
+        if (negs != nullptr) {
+          neg = (long long)negs[pos * a.n_neg + j];
+        } else if (a.num_items > 1) {
+          // K5 stream of the pointwise kernel: record pos, negative number j + 1
+          Philox4 s = fps_philox((uint32_t)pos, (uint32_t)((unsigned long long)pos >> 32),
+                                 (uint32_t)(j + 1), (uint32_t)a.step, (uint32_t)a.seed,
+                                 (uint32_t)(a.seed >> 32));
+          const unsigned long long h = ((unsigned long long)s.x << 32) | s.y;
+          neg = (long long)(h % (unsigned long long)a.num_items);
+          if (neg == (long long)item)
+            neg = (neg + 1 + (long long)((s.z % 7u) % (unsigned long long)(a.num_items - 1))) % a.num_items;
+        }
+        if (neg == (long long)item) neg = -1;   // an explicit negative equal to the positive is void
+      }
+      const bool live = neg >= 0;
+      float* vjp = bpr_row<IdT>(a.cand_table, a.cand_div, a.cand_shift, a.cand_sharded, a.cand_tab,
+                                (IdT)(live ? neg : 0), stride);
+      float4 vj[VPL];
+      float d = 0.f;
+#pragma unroll
+      for (int c = 0; c < VPL; ++c) {
+        const int q = lane + c * LPR;
+        vj[c] = (live && q < nvec) ? fps_ld_row4(vjp + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
+        d += u[c].x * (vi[c].x - vj[c].x) + u[c].y * (vi[c].y - vj[c].y) +
+             u[c].z * (vi[c].z - vj[c].z) + u[c].w * (vi[c].w - vj[c].w);
+      }
+      const float x = fps_group_sum<LPR>(d);
+      if (!live) continue;
+      const float g = a.lr / (1.f + __expf(x));   // lr * sigmoid(-x)
+      if (!(fabsf(g) <= 3.0e38f)) bad = true;      // NaN/Inf guard (Vector.scala:78-80)
+      if (lane == 0) {
+        loss_acc += fmaxf(-x, 0.f) + log1pf(expf(-fabsf(x)));   // softplus(-x), stable for any |x|
+        cnt_acc += 1.f;
+        ok_acc += x > 0.f ? 1.f : 0.f;
+      }
+      g_sum += g;
+      ++n_live;
+      float* pj = (a.cand_sharded && a.use_push_tab) ? fps_row_t<IdT>(a.push_tab, (IdT)neg) : vjp;
+#pragma unroll
+      for (int c = 0; c < VPL; ++c) {
+        const int q = lane + c * LPR;
+        if (q < nvec) {
+          du[c] = bpr_axpy(g, make_float4(vi[c].x - vj[c].x, vi[c].y - vj[c].y, vi[c].z - vj[c].z,
+                                          vi[c].w - vj[c].w), 1.f, du[c]);
+          fps_red_add4(pj + 4 * q, bpr_axpy(-g, u[c], -decay, vj[c]));   // the PUSH of v_j
+        }
+      }
+    }
+    if (n_live > 0) {
+      const float dec = decay * (float)n_live;
+      float* pi = (a.cand_sharded && a.use_push_tab) ? fps_row_t<IdT>(a.push_tab, item) : vip;
+#pragma unroll
+      for (int c = 0; c < VPL; ++c) {
+        const int q = lane + c * LPR;
+        if (q < nvec) {
+          fps_red_add4(up + 4 * q, bpr_axpy(-dec, u[c], 1.f, du[c]));       // anchor update
+          fps_red_add4(pi + 4 * q, bpr_axpy(g_sum, u[c], -dec, vi[c]));     // the PUSH of v_i
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, o);
+    cnt_acc += __shfl_xor_sync(0xffffffffu, cnt_acc, o);
+    ok_acc += __shfl_xor_sync(0xffffffffu, ok_acc, o);
+  }
+  if ((threadIdx.x & 31) == 0 && a.stats != nullptr && cnt_acc > 0.f) {
+    atomicAdd(a.stats + 0, loss_acc);
+    atomicAdd(a.stats + 1, cnt_acc);
+    atomicAdd(a.stats + 2, ok_acc);
+  }
+  if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
+}
+
+// Static pull limiter: a lane-group has up to 3 rows in flight (u, v_i, v_j), so the grid is capped at
+// max_inflight_rows / (3 * lane-groups per CTA).  `reserve_total` CTA slots stay free for the replica
+// exchange that runs next to the step (as in launch_mf of fps_core.cu).
+template <typename IdT, int LPR, int VPL, int MINB, int FMT>
+static int launch_bpr(const BprArgs& a, int max_inflight_rows, int num_sms, cudaStream_t stream) {
+  const int threads = 256;
+  const int groups_per_block = threads / LPR;
+  int occ = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fps_mf_bpr_kernel<IdT, LPR, VPL, MINB, FMT>, threads, 0);
+  if (occ < 1) occ = 1;
+  long long blocks = (long long)num_sms * occ - a.reserve_total;
+  if (blocks < num_sms) blocks = num_sms;
+  if (max_inflight_rows > 0) {
+    long long cap = max_inflight_rows / (3LL * groups_per_block);
+    if (cap < 1) cap = 1;
+    if (blocks > cap) blocks = cap;
+  }
+  long long need = (a.n_pos + groups_per_block - 1) / groups_per_block;
+  if (need < 1) need = 1;
+  if (blocks > need) blocks = need;
+  fps_mf_bpr_kernel<IdT, LPR, VPL, MINB, FMT><<<(int)blocks, threads, 0, stream>>>(a);
+  return (int)cudaGetLastError();
+}
+
+// Lane geometry of dispatch_mf (fps_core.cu): LPR lanes per row, VPL float4 per lane.
+template <typename IdT, int FMT>
+static int dispatch_bpr(const BprArgs& a, int max_inflight, int num_sms, cudaStream_t s) {
+  const int nvec = a.stride >> 2;
+  if (nvec <= 1) return launch_bpr<IdT, 1, 1, 4, FMT>(a, max_inflight, num_sms, s);
+  if (nvec <= 2) return launch_bpr<IdT, 2, 1, 4, FMT>(a, max_inflight, num_sms, s);
+  if (nvec <= 4) return launch_bpr<IdT, 4, 1, 4, FMT>(a, max_inflight, num_sms, s);
+  if (nvec <= 8) return launch_bpr<IdT, 8, 1, 4, FMT>(a, max_inflight, num_sms, s);
+  if (nvec <= 16) return launch_bpr<IdT, 16, 1, 4, FMT>(a, max_inflight, num_sms, s);
+  if (nvec <= 32) return launch_bpr<IdT, 32, 1, 4, FMT>(a, max_inflight, num_sms, s);
+  if (nvec <= 64) return launch_bpr<IdT, 32, 2, 3, FMT>(a, max_inflight, num_sms, s);
+  if (nvec <= 96) return launch_bpr<IdT, 32, 3, 2, FMT>(a, max_inflight, num_sms, s);
+  if (nvec <= 128) return launch_bpr<IdT, 32, 4, 2, FMT>(a, max_inflight, num_sms, s);
+  return -1000;  // rows wider than 512 floats
+}
+
+extern "C" int fps_mf_bpr_fused(const BprArgs* args, int id_bytes, int max_inflight_rows, int num_sms,
+                                cudaStream_t stream) {
+  if (args->n_pos <= 0 || args->n_neg <= 0) return 0;
+  if ((args->stride & 3) != 0) return -1000;
+  if (args->format == 1) return dispatch_bpr<int, 1>(*args, max_inflight_rows, num_sms, stream);
+  if (id_bytes == 4) return dispatch_bpr<int, 0>(*args, max_inflight_rows, num_sms, stream);
+  if (id_bytes == 8) return dispatch_bpr<long long, 0>(*args, max_inflight_rows, num_sms, stream);
+  return -1001;
+}

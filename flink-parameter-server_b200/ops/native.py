@@ -312,6 +312,106 @@ def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
     _bump()
 
 
+class BprArgsC(C.Structure):
+    """Mirror of ``struct BprArgs`` (csrc/fps_mf_bpr.cu)."""
+
+    _fields_ = [
+        ("users", C.c_void_p), ("items", C.c_void_p), ("ratings", C.c_void_p), ("negatives", C.c_void_p),
+        ("n_pos", C.c_longlong), ("n_neg", C.c_int), ("format", C.c_int),
+        ("num_items", C.c_longlong), ("seed", C.c_ulonglong), ("step", C.c_ulonglong),
+        ("lr", C.c_float), ("reg", C.c_float),
+        ("anchor_table", C.c_void_p), ("anchor_div", C.c_int), ("anchor_shift", C.c_int),
+        ("anchor_sharded", C.c_int), ("cand_sharded", C.c_int), ("anchor_tab", ShardTableC),
+        ("cand_table", C.c_void_p), ("cand_div", C.c_int), ("cand_shift", C.c_int), ("cand_tab", ShardTableC),
+        ("use_push_tab", C.c_int), ("stride", C.c_int), ("push_tab", ShardTableC),
+        ("stats", C.c_void_p), ("nan_flag", C.c_void_p), ("reserve_total", C.c_int), ("pad_", C.c_int),
+    ]
+
+
+def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Optional[torch.Tensor],
+                 anchor_table, cand_table, lr: float, reg: float = 0.0, *,
+                 negatives: Optional[torch.Tensor] = None, n_neg: int = 1, num_items: int = 0,
+                 seed: int = 0, step: int = 0, anchor_div: int = 1, cand_div: int = 1,
+                 stats: Optional[torch.Tensor] = None, nan_flag: Optional[torch.Tensor] = None,
+                 max_inflight_rows: int = 0, push_tab: Optional[ShardTableC] = None,
+                 reserve_total: int = 0) -> None:
+    """Fused pairwise (BPR) pull + SGD + push, one ``(anchor, positive, negative)`` triple per update
+    (csrc/fps_mf_bpr.cu).  ``users`` are the anchor ids, ``items`` the positive candidates; records with
+    ``rating <= 0`` are skipped.  ``items=None``: ``users`` holds packed64 records (:func:`pack_ratings`).
+
+    ``anchor_table`` / ``cand_table``: a worker-local ``[rows, stride]`` float32 tensor (row of id =
+    ``id // anchor_div`` / ``id // cand_div``) or a :class:`ShardTableC`.  ``push_tab`` (with a
+    ShardTable ``cand_table``) receives the candidate deltas instead of ``cand_table``.
+
+    ``negatives``: ``[n_pos, n]`` ids of the same dtype as ``users`` (int32 for packed64), ``-1`` voids a
+    triple.  Without it ``n_neg`` negatives per positive are drawn in the kernel, uniform over
+    ``[0, num_items)`` and never the positive.  ``stats`` (float32 ``[3]``) accumulates the softplus loss
+    sum, the number of triples and the number with ``x > 0``.  ``max_inflight_rows`` caps the grid so that
+    at most that many rows are being pulled at once (3 per lane-group).  ``reserve_total``: CTA slots
+    the grid leaves free for a kernel running next to it (the replica exchange)."""
+    _req(users, "users")
+    packed = items is None
+    if packed:
+        if users.dtype != torch.int64:
+            raise TypeError("packed rating records must be an int64 tensor (see pack_ratings)")
+        id_dtype = torch.int32
+    else:
+        _req(items, "items"); _req(ratings, "ratings", torch.float32)
+        if users.dtype != items.dtype:
+            raise TypeError("users and items must share an integer dtype")
+        if items.numel() != users.numel() or ratings.numel() != users.numel():
+            raise ValueError("users, items and ratings must have the same length")
+        id_dtype = users.dtype
+    n_pos = users.numel()
+    a = BprArgsC()
+    strides = []
+    for name, tab, div in (("anchor", anchor_table, anchor_div), ("cand", cand_table, cand_div)):
+        if isinstance(tab, ShardTableC):
+            setattr(a, f"{name}_tab", tab); setattr(a, f"{name}_sharded", 1)
+            strides.append(int(tab.stride))
+        else:
+            _req(tab, f"{name}_table", torch.float32)
+            setattr(a, f"{name}_table", tab.data_ptr())
+            setattr(a, f"{name}_div", int(div)); setattr(a, f"{name}_shift", log2_or_neg(int(div)))
+            strides.append(int(tab.shape[1]))
+    if strides[0] != strides[1]:
+        raise ValueError("anchor table stride must equal candidate table stride")
+    a.stride = strides[0]
+    if push_tab is not None:
+        if not a.cand_sharded:
+            raise ValueError("push_tab needs a ShardTable cand_table")
+        if int(push_tab.stride) != a.stride:
+            raise ValueError("push table stride must equal candidate table stride")
+        a.push_tab = push_tab; a.use_push_tab = 1
+    if negatives is not None:
+        _req(negatives, "negatives", id_dtype)
+        if negatives.dim() != 2 or negatives.shape[0] != n_pos:
+            raise ValueError(f"negatives must be [{n_pos}, n]")
+        a.negatives = negatives.data_ptr(); a.n_neg = int(negatives.shape[1])
+    else:
+        if int(n_neg) < 1:
+            raise ValueError("n_neg must be >= 1 when negatives are sampled")
+        a.n_neg = int(n_neg)
+    if stats is not None:
+        _req(stats, "stats", torch.float32)
+        if stats.numel() < 3:
+            raise ValueError("stats must hold 3 floats")
+        a.stats = stats.data_ptr()
+    if nan_flag is not None:
+        _req(nan_flag, "nan_flag", torch.int32)
+        a.nan_flag = nan_flag.data_ptr()
+    a.users = users.data_ptr()
+    a.items = None if packed else items.data_ptr()
+    a.ratings = None if packed else ratings.data_ptr()
+    a.format = 1 if packed else 0
+    a.n_pos = n_pos; a.num_items = int(max(num_items, 1))
+    a.seed = seed & (2**64 - 1); a.step = int(step)
+    a.lr = float(lr); a.reg = float(reg); a.reserve_total = int(reserve_total)
+    _check(lib().fps_mf_bpr_fused(C.byref(a), 4 if packed else _id_bytes(users), int(max_inflight_rows),
+                                  sm_count(users.device.index), _stream()), "mf_bpr_fused")
+    _bump()
+
+
 def init_rows_f64(rows: torch.Tensor, dim: int, shard: int, num_shards: int, mode: int, div: int, seed: int,
                   lo: float, hi: float) -> None:
     """Philox init-by-id of fp64 rows ``[n, stride_doubles]`` (53-bit uniforms)."""

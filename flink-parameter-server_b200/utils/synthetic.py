@@ -34,3 +34,35 @@ def lowrank_ratings(users: torch.Tensor, items: torch.Tensor, rank: int = 8, see
     for f in range(rank):
         r += hashed_uniform(users, f, 2 * seed + 1) * hashed_uniform(items, f, 2 * seed + 2)
     return r * (scale / rank ** 0.5)
+
+
+def lowrank_implicit(num_users: int, num_items: int, per_user: int, held_out: int, seed: int,
+                     beta: float = 4.0, rank: int = 8):
+    """Implicit feedback with a learnable ranking: every user "consumes" ``per_user`` distinct items, the
+    Gumbel top-``per_user`` of ``beta * lowrank_ratings(u, i)`` (a draw without replacement with
+    probabilities ~ ``exp(beta * r)``), and ``held_out`` of them, chosen at random, are kept apart.
+
+    Returns int64 CPU tensors ``(train_users, train_items, test_users, test_items)``; the train pairs are
+    in a random stream order, the test pairs ordered by user.  A pure function of its arguments; it
+    scores every (user, item) pair, so it is meant for small sizes (about 10^4 x 10^4)."""
+    if not 0 <= held_out < per_user <= num_items:
+        raise ValueError("need 0 <= held_out < per_user <= num_items")
+    g = torch.Generator().manual_seed(int(seed))
+    scale = 1.5 / rank ** 0.5                  # lowrank_ratings as a product of its per-id factors
+    iid = torch.arange(num_items)
+    B = torch.stack([hashed_uniform(iid, f, 2 * seed + 2) for f in range(rank)], 1)
+    tr_u, tr_i, te_u, te_i = [], [], [], []
+    for lo in range(0, num_users, 1024):
+        uid = torch.arange(lo, min(lo + 1024, num_users))
+        A = torch.stack([hashed_uniform(uid, f, 2 * seed + 1) for f in range(rank)], 1)
+        u01 = torch.rand((uid.numel(), num_items), generator=g).clamp_(1e-12, 1.0 - 1e-7)
+        keys = beta * scale * (A @ B.T) - torch.log(-torch.log(u01))
+        top = keys.topk(per_user, dim=1).indices
+        order = torch.rand((uid.numel(), per_user), generator=g).argsort(1)
+        top = top.gather(1, order)
+        users = uid[:, None].expand(-1, per_user)
+        te_u.append(users[:, :held_out].reshape(-1)); te_i.append(top[:, :held_out].reshape(-1))
+        tr_u.append(users[:, held_out:].reshape(-1)); tr_i.append(top[:, held_out:].reshape(-1))
+    tr_u, tr_i = torch.cat(tr_u), torch.cat(tr_i)
+    perm = torch.randperm(tr_u.numel(), generator=g)
+    return tr_u[perm], tr_i[perm], torch.cat(te_u), torch.cat(te_i)
