@@ -12,6 +12,11 @@ Records, in one process:
 * A/B rows: the step's device time with 16 MB and 4 MB item buckets and without the deal, the configurations
   alternated round by round, with the spread over the rounds.  (``DeviceOnlineMF.step`` deals a micro-batch only
   when it has more records than the table has rows, so at this shape the bucket rows run without the deal too.)
+
+``--window`` records the step window instead (``DeviceOnlineMF(step_window=8)``, fps_mf_window.cu), written to
+``profiles/h100_mf_step_window.json`` by default: device times of the staging copies and of the drain for each
+kernel variant (CUDA events and ``torch.profiler``), the bytes model of a windowed step next to them, TB/s against
+the ``copy_`` ceiling, and A/B rows of the windowed and the per-launch step alternated round by round.
 """
 from __future__ import annotations
 
@@ -95,6 +100,8 @@ def kernel_class(name: str) -> str:
         return "bucket"
     if "mf_sgd_fused" in n:
         return "fused"
+    if "mf_window" in n:
+        return "drain"
     return "other"
 
 
@@ -113,7 +120,7 @@ def profile(model, steps, n_steps):
     ev.sort(key=lambda e: e["ts"])
     per = {}
     for e in ev:
-        c = "memset" if e["cat"] == "gpu_memset" else kernel_class(e["name"])
+        c = {"gpu_memset": "memset", "gpu_memcpy": "staging_copy"}.get(e["cat"]) or kernel_class(e["name"])
         if c == "other" and ("zero" in e["name"].lower() or "fill" in e["name"].lower()):
             c = "stats_reset"
         d = per.setdefault(c, {"count": 0, "us": 0.0, "names": set()})
@@ -164,14 +171,106 @@ def bytes_model(n_per_mb, row_bytes, record_bytes, sort_pass_bytes):
     }
 
 
+WINDOW_VARIANTS = {"p4_3cta": "0", "p8_2cta": "1"}   # FPS_MF_WINDOW_VARIANT: user rows prefetched, CTAs/SM
+
+
+def window_bytes_model(step, row_bytes):
+    """Bytes one windowed step moves, computed from the step's records (packed64)."""
+    rec = torch.cat(step)
+    n = rec.numel()
+    touched = int(torch.unique((rec >> 16) & 0x3FFFFF).numel())
+    staging = 2 * 8 * n                        # D2D copy into the staging slots: read + write
+    drain_records = 8 * n                      # the drain reads every staged record once
+    slot_table = 3 * 8 * n                     # T entry: atomicExch, chain read, reset (may stay in L2)
+    users = 2 * row_bytes * n                  # every user row read and written once
+    items = 2 * row_bytes * touched            # every touched item row read and written once
+    return {"records": n, "touched_item_rows": touched, "row_bytes": row_bytes,
+            "staging_copy_bytes": staging, "drain_record_bytes": drain_records, "slot_table_bytes": slot_table,
+            "user_rows_bytes": users, "item_rows_bytes": items,
+            "drain_bytes": users + items + drain_records + slot_table,
+            "per_launch_bytes": 2 * row_bytes * n * 2 + 8 * n,
+            "note": "computed from shapes and the step's item ids; slot-table and bitmap traffic are upper bounds "
+                    "(they may be served by L2)"}
+
+
+def window_split(model, steps, n_steps):
+    """Device time of the staging copies and of the drain of each step, separately (CUDA events)."""
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+    stage_ms, drain_ms = [], []
+    for s in range(n_steps):
+        model.stats.zero_()
+        ev[0].record()
+        for b in steps[s % len(steps)]:
+            model._stage(b, None, None)
+        ev[1].record()
+        model._drain()
+        ev[2].record()
+        torch.cuda.synchronize()
+        stage_ms.append(ev[0].elapsed_time(ev[1]))
+        drain_ms.append(ev[1].elapsed_time(ev[2]))
+    return statistics.median(stage_ms), statistics.median(drain_ms)
+
+
+def window_main(a, res, steps, sizes, DeviceOnlineMF):
+    ref = DeviceOnlineMF(USERS, ITEMS, K, learning_rate=0.01, seed=1234, step_window=0)
+    win = DeviceOnlineMF(USERS, ITEMS, K, learning_rate=0.01, seed=1234, step_window=8)
+    row_bytes = win._items.stride * 4
+    bm = window_bytes_model(steps[0], row_bytes)
+    ceiling = res["hbm_copy"]["tb_per_s"]
+    res["window"] = {"step_window": win.step_window, "bytes_model": bm, "variants": {}}
+    arms = {"per_launch": (ref, None)}
+    arms.update({"window_" + v: (win, code) for v, code in WINDOW_VARIANTS.items()})
+    for m, code in arms.values():               # warm every kernel
+        if code is not None:
+            os.environ["FPS_MF_WINDOW_VARIANT"] = code
+        timed(m, steps, a.warmup, 0)
+    for v, code in WINDOW_VARIANTS.items():
+        os.environ["FPS_MF_WINDOW_VARIANT"] = code
+        stage, drain = window_split(win, steps, a.steps)
+        prof = profile(win, steps, 4)
+        res["window"]["variants"][v] = {
+            "staging_ms_per_step": stage, "drain_ms_per_step": drain,
+            "drain_tb_per_s": bm["drain_bytes"] / (drain * 1e-3) / 1e12,
+            "drain_share_of_copy_ceiling": bm["drain_bytes"] / (drain * 1e-3) / 1e12 / ceiling,
+            "staging_tb_per_s": bm["staging_copy_bytes"] / (stage * 1e-3) / 1e12,
+            "profile": prof}
+    ms = {c: [] for c in arms}
+    names = list(arms)
+    for r in range(a.rounds):
+        for c in (names if r % 2 == 0 else names[::-1]):
+            m, code = arms[c]
+            if code is not None:
+                os.environ["FPS_MF_WINDOW_VARIANT"] = code
+            ms[c].append(timed(m, steps, a.steps, r))
+    os.environ.pop("FPS_MF_WINDOW_VARIANT", None)
+    base = statistics.median(ms["per_launch"])
+    res["ab"] = {c: {"ms_per_step": v, "median_ms": statistics.median(v), "min_ms": min(v), "max_ms": max(v),
+                     "updates_per_s_median": BATCH / (statistics.median(v) * 1e-3),
+                     "speedup_vs_per_launch": base / statistics.median(v)}
+                 for c, v in ms.items()}
+    res["ab_note"] = (f"{a.rounds} rounds x {a.steps} steps per arm, arms alternated (reversed order every other "
+                      "round); device time per step from CUDA events, stats reset + staging + drain included")
+    res["per_launch_profile"] = profile(ref, steps, 4)
+    res["per_launch_profile"]["bytes_tb_per_s"] = bm["per_launch_bytes"] / (
+        res["per_launch_profile"]["busy_us_per_step"] * 1e-6) / 1e12
+    for m in (win, ref):
+        m.check_finite()
+        m.close()
+    return {c: res["ab"][c]["median_ms"] for c in names}
+
+
 def main():
     p = argparse.ArgumentParser()
-    p.add_argument("--out", default=os.path.join(REPO, "profiles", "h100_mf_step_breakdown.json"))
+    p.add_argument("--out", default=None)
+    p.add_argument("--window", action="store_true", help="record the step window (see the module docstring)")
     p.add_argument("--rounds", type=int, default=5)
     p.add_argument("--steps", type=int, default=40)
     p.add_argument("--warmup", type=int, default=4)
     p.add_argument("--configs", default=",".join(CONFIGS))
     a = p.parse_args()
+    if a.out is None:
+        a.out = os.path.join(REPO, "profiles", "h100_mf_step_window.json" if a.window
+                             else "h100_mf_step_breakdown.json")
 
     torch.cuda.set_device(0)
     dev = torch.device("cuda", 0)
@@ -183,7 +282,15 @@ def main():
     res["hbm_copy"] = hbm_ceiling()
     steps, sizes = bench_batches(native, dev)
     res["shape"]["micro_batches_per_step"] = len(sizes)
-    model = DeviceOnlineMF(USERS, ITEMS, K, learning_rate=0.01, seed=1234, item_blocking=True)
+    if a.window:
+        summary = window_main(a, res, steps, sizes, DeviceOnlineMF)
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(res, f, indent=1)
+        print(json.dumps(summary))
+        return
+    model = DeviceOnlineMF(USERS, ITEMS, K, learning_rate=0.01, seed=1234, item_blocking=True,
+                           step_window=0)
     row_bytes = model.items.stride * 4
 
     names = [c for c in a.configs.split(",") if c in CONFIGS]

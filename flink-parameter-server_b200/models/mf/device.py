@@ -34,6 +34,46 @@ ERR_PLAIN = 1    # textbook SGD:     e = r - u.v
 
 DEFAULT_DEVICE_PULL_LIMIT = 0  # 0 = as many row slots in flight as the GPU can hold
 
+L2_TABLE_BYTES = 48 << 20      # item tables above this do not stay in an H100's 50 MB L2 between launches
+WINDOW_BUDGET = 256 << 20      # device memory of the step window: slot table + record staging
+WINDOW_BYTES_PER_ROW = 8 + 12  # per item row and window slot: one slot-table entry + one int32-array record
+WINDOW_MAX_STRIDE = 128        # floats per row the window kernel handles (k <= 128)
+
+
+def step_window_size(step_window: Optional[int], *, world: int, item_cache: bool, loss: str, table_rows: int,
+                     stride: int, env: Optional[str] = None) -> int:
+    """Micro-batches per step window of :class:`DeviceOnlineMF` (0 = off).
+
+    ``None`` = auto: on for one worker without an item cache whose item table exceeds the L2 (where every
+    micro-batch re-reads it from HBM), unless ``FPS_STEP_WINDOW=0`` (``env``).  ``0`` / ``1`` = off, ``n >= 2`` =
+    at most ``n`` (and at most ``native.WINDOW_MAX``).  The slot table and the staging area take
+    ``W * table_rows * 20`` bytes, capped at ``WINDOW_BUDGET``: ``W`` is lowered to fit, and the window is off
+    below 2."""
+    if world != 1 or item_cache or loss != "pointwise" or stride > WINDOW_MAX_STRIDE or table_rows < 1:
+        return 0
+    if step_window is None:
+        if env == "0" or table_rows * stride * 4 <= L2_TABLE_BYTES:
+            return 0
+        w = native.WINDOW_MAX
+    else:
+        w = min(int(step_window), native.WINDOW_MAX)
+    w = min(w, WINDOW_BUDGET // (table_rows * WINDOW_BYTES_PER_ROW))
+    return w if w >= 2 else 0
+
+
+def step_windowable(*, neg: int, output_ring, pull_limit: int, credits, kernel: Optional[str], kernel_env: str,
+                    reg_variant_env: Optional[str], l2_hints: bool, packed: bool, dtypes: Tuple, n_records: int,
+                    table_rows: int, on_gpu: bool, capturing: bool) -> bool:
+    """Whether one pointwise ``step()`` can join the window: the per-launch path it replaces is the default
+    register-staged kernel (no negatives, output ring, pull limiter, L2 hints or other variant) on int32 or
+    packed64 records, no more of them than the table has rows, outside CUDA-graph capture."""
+    if neg != 0 or output_ring is not None or pull_limit != 0 or credits is not None or l2_hints:
+        return False
+    if (kernel or kernel_env) != "reg" or reg_variant_env not in (None, "0") or capturing or not on_gpu:
+        return False
+    ok_dtypes = dtypes == (torch.int64,) if packed else dtypes == (torch.int32, torch.int32, torch.float32)
+    return ok_dtypes and n_records <= table_rows
+
 
 class DeviceOnlineMF:
     def __init__(self, num_users: int, num_items: int, num_factors: int = 10,
@@ -46,10 +86,16 @@ class DeviceOnlineMF:
                  sync_interval_ms: Optional[float] = None, item_blocking: Optional[bool] = None,
                  block_bytes: int = 16 << 20, flush_count: Optional[int] = None,
                  flush_require: str = "any", replica_own_inplace: Optional[bool] = None,
-                 output_ring=None, loss: str = "pointwise", regularization: float = 0.0):
+                 output_ring=None, loss: str = "pointwise", regularization: float = 0.0,
+                 step_window: Optional[int] = None):
         """``loss="bpr"``: pairwise (Bayesian Personalised Ranking) updates, each positive rating paired
         with ``negative_sample_rate`` negatives (sampled) or with the ``negatives=`` of :meth:`step`;
-        ``regularization`` is its L2 weight.  The pointwise loss has no regulariser."""
+        ``regularization`` is its L2 weight.  The pointwise loss has no regulariser.
+
+        ``step_window``: how many micro-batches :meth:`step` may defer and then apply in one item-major pass
+        (see :meth:`step` and :func:`step_window_size`; ``None`` = auto, ``0`` = off)."""
+        self._pending = []           # staged micro-batches of the step window: (records, format)
+        self.step_window = 0
         if loss not in ("pointwise", "bpr"):
             raise ValueError(f"loss must be 'pointwise' or 'bpr', got {loss!r}")
         self.loss, self.reg = loss, float(regularization)
@@ -87,19 +133,19 @@ class DeviceOnlineMF:
         self.output_ring = output_ring     # E5: per-update (user, vector) output stream (runtime/output_ring.py)
         with torch.cuda.device(self.device):
             # parameter server: item vectors, sharded item % psParallelism
-            self.items = ShardedTable(num_items, num_factors, partition="hash", group=group,
+            self._items = ShardedTable(num_items, num_factors, partition="hash", group=group,
                                       device=self.device, init="uniform",
                                       init_range=(range_min, range_max), seed=seed * 2 + 1,
                                       track_touched=track_touched)
             # worker-local state: vectors of the users this worker owns (user % W == rank)
             n_local = -(-self.num_users // self.world)
-            self.users = torch.empty((n_local, self.items.stride), dtype=torch.float32,
+            self._users = torch.empty((n_local, self._items.stride), dtype=torch.float32,
                                      device=self.cuda_device)
-            native.init_rows(self.users, self.k, self.rank, self.world, native.PART_HASH, n_local,
+            native.init_rows(self._users, self.k, self.rank, self.world, native.PART_HASH, n_local,
                              seed * 2 + 2, range_min, range_max)
             # pointwise: [sum (r - u.v)^2, updates]; BPR: [sum softplus(-x), triples, triples with x > 0]
-            self.stats = torch.zeros(3 if loss == "bpr" else 2, dtype=torch.float32, device=self.cuda_device)
-            self.nan_flag = torch.zeros(1, dtype=torch.int32, device=self.cuda_device)
+            self._stats = torch.zeros(3 if loss == "bpr" else 2, dtype=torch.float32, device=self.cuda_device)
+            self._nan_flag = torch.zeros(1, dtype=torch.int32, device=self.cuda_device)
             # K5: per-user memory of recently seen items (userMemory of the reference, default 128
             # there; 0 here = sample uniformly inside the fused kernel, rejecting only the positive)
             self.user_memory = int(user_memory) if self.neg > 0 else 0
@@ -122,13 +168,13 @@ class DeviceOnlineMF:
         self.sync_interval_ms = sync_interval_ms
         self.flush_count, self.flush_require = flush_count, flush_require
         self._own_inplace = replica_own_inplace
-        self.replica = (ReplicaCache(self.items, self.sync_every, sync_interval_ms,
+        self.replica = (ReplicaCache(self._items, self.sync_every, sync_interval_ms,
                                      require=flush_require, flush_count=flush_count,
                                      own_inplace=replica_own_inplace)
                         if self.item_cache else None)
         # ---- L2 blocking: deal each micro-batch into buckets of <= 16 MB of item rows (fps_bucket.cu) ----
         # only where the item rows are read from local HBM (single GPU, or the local replica)
-        row_bytes = self.items.stride * 4
+        row_bytes = self._items.stride * 4
         if item_blocking is None:
             item_blocking = ((self.world == 1 or self.item_cache) and self.num_items * row_bytes > (48 << 20)
                              and (self.neg == 0 or self.user_memory > 0)
@@ -140,7 +186,7 @@ class DeviceOnlineMF:
         self.block_shift = max(0, per_bucket.bit_length() - 1)
         # buckets are ranges of rows of the table the fused kernel reads: the item shard (N = 1) or the
         # owner-major replica (row = owner * rows_per_shard + slot)
-        table_rows = self.items.rows_per_shard * self.world if self.item_cache else self.num_items
+        table_rows = self._items.rows_per_shard * self.world if self.item_cache else self.num_items
         self._table_rows = table_rows
         while -(-table_rows >> self.block_shift) > native.BUCKET_MAX:
             self.block_shift += 1
@@ -149,11 +195,97 @@ class DeviceOnlineMF:
             with torch.cuda.device(self.device):
                 self._bucket_scratch = torch.zeros(2 * native.BUCKET_MAX, dtype=torch.int32,
                                                    device=self.cuda_device)
-        self.items.barrier()
+        # ---- step window (fps_mf_window.cu): buffers allocated by the first windowed step ----------------
+        self.step_window = step_window_size(step_window, world=self.world, item_cache=self.item_cache,
+                                            loss=self.loss, table_rows=self.num_items, stride=self._items.stride,
+                                            env=os.environ.get("FPS_STEP_WINDOW"))
+        self._win = None
+        self._graph_capture = False
+        self._per_launch = False
+        self._items.barrier()
+
+    # -- model state: every read applies the pending step window first ------------------------------------
+    @property
+    def stats(self) -> torch.Tensor:
+        self._drain()
+        return self._stats
+
+    @property
+    def users(self) -> torch.Tensor:
+        self._drain()
+        return self._users
+
+    @property
+    def items(self) -> ShardedTable:
+        self._drain()
+        return self._items
+
+    @property
+    def nan_flag(self) -> torch.Tensor:
+        self._drain()
+        return self._nan_flag
+
+    def _windowable(self, users, items, ratings) -> bool:
+        if self.step_window < 2 or self._graph_capture or self._per_launch:
+            return False
+        packed = items is None
+        return step_windowable(
+            neg=self.neg, output_ring=self.output_ring, pull_limit=self.pull_limit, credits=self.credits,
+            kernel=self.kernel, kernel_env=os.environ.get("FPS_MF_KERNEL", "reg"),
+            reg_variant_env=os.environ.get("FPS_MF_REG_VARIANT"), l2_hints=self.l2_hints, packed=packed,
+            dtypes=(users.dtype,) if packed else (users.dtype, items.dtype, ratings.dtype),
+            n_records=users.numel(), table_rows=self.num_items, on_gpu=users.is_cuda,
+            capturing=torch.cuda.is_current_stream_capturing())
+
+    def _stage(self, users, items, ratings) -> None:
+        """Copy one micro-batch into the next slot of the device staging area (stream-ordered; the caller may
+        reuse its tensors at once).  No kernel runs."""
+        if self._win is None:
+            rows, w = self.num_items, self.step_window
+            slot_bytes = -(-rows * 12 // 256) * 256
+            with torch.cuda.device(self.device):
+                dev = self.cuda_device
+                self._win = {
+                    "slot_bytes": slot_bytes,
+                    "stage": torch.empty(w * slot_bytes, dtype=torch.uint8, device=dev),
+                    "slots": torch.full((w, rows), -1, dtype=torch.int64, device=dev),   # item-major slot table
+                    "user_bits": torch.zeros(-(-self._users.shape[0] // 32), dtype=torch.int32, device=dev),
+                    "ctl": torch.zeros(2 * native.WINDOW_MAX, dtype=torch.int32, device=dev),
+                    "slot_stats": torch.zeros((w, 2), dtype=torch.float32, device=dev),
+                }
+        j = len(self._pending)
+        n = users.numel()
+        sb = self._win["slot_bytes"]
+        slot = self._win["stage"][j * sb:(j + 1) * sb]
+        if items is None:
+            slot[:8 * n].view(torch.int64).copy_(users.reshape(-1), non_blocking=True)
+        else:
+            ids = slot[:12 * n].view(torch.int32)
+            ids[:n].copy_(users.reshape(-1), non_blocking=True)
+            ids[n:2 * n].copy_(items.reshape(-1), non_blocking=True)
+            ids[2 * n:].view(torch.float32).copy_(ratings.reshape(-1), non_blocking=True)
+        self._pending.append((n, 1 if items is None else 0))
+        self.step_no += 1
+        METRICS.inc("mf_ratings", n)
+
+    def _drain(self) -> int:
+        """Apply the staged micro-batches in order (one launch); returns how many there were."""
+        n = len(self._pending)
+        if n == 0:
+            return 0
+        counts, fmts = zip(*self._pending)
+        self._pending = []
+        w = self._win
+        native.mf_window_drain(w["stage"], w["slot_bytes"], counts, fmts, self._users, self._items.local, self.lr,
+                               self.err_mode, w["slots"], w["user_bits"], w["ctl"], self._stats, w["slot_stats"],
+                               self._nan_flag)
+        return n
 
     # ------------------------------------------------------------------------------------
     def flush(self) -> None:
-        """Item-cache mode: push every pending local delta to the master shards and wait for it."""
+        """Apply the pending step window; item-cache mode: push every pending local delta to the master shards
+        and wait for it."""
+        self._drain()
         if self.replica is not None:
             self.replica.flush()
 
@@ -161,7 +293,21 @@ class DeviceOnlineMF:
              ratings: Optional[torch.Tensor] = None, negatives: Optional[torch.Tensor] = None) -> None:
         """Process one micro-batch of ratings whose users belong to this worker (async SGD).
         ``step(packed)`` with a single int64 tensor takes packed64 records (``native.pack_ratings``).
-        ``negatives`` (``loss="bpr"`` only): ``[n, m]`` item ids paired with each rating, ``-1`` = none."""
+        ``negatives`` (``loss="bpr"`` only): ``[n, m]`` item ids paired with each rating, ``-1`` = none.
+
+        Lazy with a step window (``step_window``): an eligible micro-batch (:func:`step_windowable`) is only
+        copied into a device staging slot -- the caller may reuse its tensors at once -- and the window is
+        applied, in order and in one launch, before any observation of the model (``stats``, ``users``,
+        ``items``, ``nan_flag``, :meth:`flush`, :meth:`predict`, :meth:`save`, :meth:`check_finite`, ...), before
+        an ineligible step, and when it is full.  The tables then equal, bitwise, one fused launch per
+        micro-batch whenever each micro-batch has distinct users and distinct items; a micro-batch with a user
+        or an item twice is applied on its own, as racy as the per-launch path."""
+        if self.loss == "pointwise" and negatives is None and self._windowable(users, items, ratings):
+            self._stage(users, items, ratings)
+            if len(self._pending) >= self.step_window:
+                self._drain()
+            return
+        self._drain()
         if self.loss == "bpr":
             self._step_bpr(users, items, ratings, negatives)
             return
@@ -185,28 +331,28 @@ class DeviceOnlineMF:
         # mode always deals: the bucket histogram feeds its flush policy.
         revisits = self.item_cache or n_records * (1 + neg) > self._table_rows
         if self.item_blocking and self.block_buckets > 1 and revisits:
-            hashed = self.item_cache and self.items.mode == native.PART_HASH
+            hashed = self.item_cache and self._items.mode == native.PART_HASH
             fed = hashed
             users, items, ratings = native.bucket_by_item(
                 users, items, ratings, self.block_shift, self.block_buckets, self._bucket_scratch,
-                num_shards=self.world if hashed else 1, rows_per_shard=self.items.rows_per_shard,
+                num_shards=self.world if hashed else 1, rows_per_shard=self._items.rows_per_shard,
                 pending=self.replica.pending if hashed else None)
         if self.item_cache:
             # policy + exchange kernels of this micro-batch go first (side stream): their CTAs take the
             # slots the training grid leaves free
             self.replica.after_step(n_records * (1 + neg), fed=fed)
-            native.mf_sgd_fused(users, items, ratings, self.users, self.world, self.replica.table_c,
+            native.mf_sgd_fused(users, items, ratings, self._users, self.world, self.replica.table_c,
                                 self.lr, err_mode=self.err_mode, neg_rate=neg,
                                 num_items=self.num_items, seed=self.seed, step=self.step_no,
-                                stats=self.stats, nan_flag=self.nan_flag,
+                                stats=self._stats, nan_flag=self._nan_flag,
                                 max_inflight_rows=self.pull_limit, kernel="reg", l2_hints=self.l2_hints,
                                 reserve_total=self.replica.reserve_total(), output=out_args,
                                 credits=self.credits)
         else:
-            native.mf_sgd_fused(users, items, ratings, self.users, self.world, self.items.table_c,
+            native.mf_sgd_fused(users, items, ratings, self._users, self.world, self._items.table_c,
                                 self.lr, err_mode=self.err_mode, neg_rate=neg,
                                 num_items=self.num_items, seed=self.seed, step=self.step_no,
-                                stats=self.stats, nan_flag=self.nan_flag,
+                                stats=self._stats, nan_flag=self._nan_flag,
                                 max_inflight_rows=self.pull_limit, kernel=self.kernel,
                                 l2_hints=self.l2_hints, output=out_args, credits=self.credits)
         if ring is not None:               # device-side count / timer policy + flush to the pinned host ring
@@ -236,14 +382,14 @@ class DeviceOnlineMF:
         if self.output_ring is not None:
             raise ValueError("the per-update output ring is not supported with loss='bpr'")
         n_pos = users.numel()
-        cand, reserve = self.items.table_c, 0
+        cand, reserve = self._items.table_c, 0
         if self.item_cache:
             # uniform per-destination counts feed the flush policy (BPR batches are not dealt into buckets)
             self.replica.after_step(n_pos * n, fed=False)
             cand, reserve = self.replica.table_c, self.replica.reserve_total()
-        native.mf_bpr_fused(users, items, ratings, self.users, cand, self.lr, self.reg, negatives=negatives,
+        native.mf_bpr_fused(users, items, ratings, self._users, cand, self.lr, self.reg, negatives=negatives,
                             n_neg=n, num_items=self.num_items, seed=self.seed, step=self.step_no,
-                            anchor_div=self.world, stats=self.stats, nan_flag=self.nan_flag,
+                            anchor_div=self.world, stats=self._stats, nan_flag=self._nan_flag,
                             max_inflight_rows=self.pull_limit, reserve_total=reserve)
         self.step_no += 1
         METRICS.inc("mf_ratings", n_pos)
@@ -253,7 +399,9 @@ class DeviceOnlineMF:
 
         Returns ``(static_inputs, replay)``: copy the next batch into ``static_inputs`` (device
         tensors) and call ``replay()``; the captured graph contains the stats reset and the fused
-        kernel, so one ``cudaGraphLaunch`` replaces the Python + ctypes launch path."""
+        kernel, so one ``cudaGraphLaunch`` replaces the Python + ctypes launch path.  The graph holds the
+        per-launch kernel: ``replay()`` applies a pending step window first."""
+        self._drain()
         dev = self.cuda_device
         if packed:
             static = (torch.zeros(batch_size, dtype=torch.int64, device=dev),)
@@ -263,15 +411,23 @@ class DeviceOnlineMF:
                       torch.zeros(batch_size, dtype=torch.float32, device=dev))
         s = torch.cuda.Stream(device=dev)
         s.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(s):
-            for _ in range(2):  # warm up outside capture
-                self.stats.zero_(); self.step(*static)
-        torch.cuda.current_stream(dev).wait_stream(s)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=s):
-            self.stats.zero_()
-            self.step(*static)
-        return static, graph.replay
+        self._graph_capture = True       # warm-up and capture take the per-launch path
+        try:
+            with torch.cuda.stream(s):
+                for _ in range(2):  # warm up outside capture
+                    self._stats.zero_(); self.step(*static)
+            torch.cuda.current_stream(dev).wait_stream(s)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, stream=s):
+                self._stats.zero_()
+                self.step(*static)
+        finally:
+            self._graph_capture = False
+
+        def replay():
+            self._drain()
+            graph.replay()
+        return static, replay
 
     def fit_stream(self, host_batches: Iterable[Sequence[torch.Tensor]],
                    loss_every: int = 1):
@@ -280,17 +436,23 @@ class DeviceOnlineMF:
         Yields one host-side ``(sum_sq_err, n_updates)`` per micro-batch (device -> host read of
         the step's result), lagging the launch by one step so copies, kernels and reads overlap.
         With ``loss="bpr"`` the pair is ``(sum softplus(-x), n_triples)``.
+        It reads the loss after every micro-batch, so it takes the per-launch path (no step window).
         """
+        self._drain()
         pf = DevicePrefetcher(host_batches, self.cuda_device, depth=2)
         self.prefetcher = pf
         pending = []
-        ring = [torch.empty(self.stats.numel(), dtype=torch.float32).pin_memory() for _ in range(4)]
+        ring = [torch.empty(self._stats.numel(), dtype=torch.float32).pin_memory() for _ in range(4)]
         i = 0
         for batch in pf:
-            self.stats.zero_()
-            self.step(*batch)
+            self._stats.zero_()
+            self._per_launch = True
+            try:
+                self.step(*batch)
+            finally:
+                self._per_launch = False
             host = ring[i % len(ring)]
-            host.copy_(self.stats, non_blocking=True)
+            host.copy_(self._stats, non_blocking=True)
             ev = torch.cuda.Event()
             ev.record()
             pending.append((host, ev))
@@ -309,20 +471,21 @@ class DeviceOnlineMF:
         """u.v for (user, item) pairs whose users are local (pull fused with the dot)."""
         self.flush()
         slots = (users.to(torch.int64) // self.world)
-        local = self.users[slots].contiguous()
-        return self.items.pull_dot(items, local)
+        local = self._users[slots].contiguous()
+        return self._items.pull_dot(items, local)
 
     def user_vectors(self) -> Tuple[torch.Tensor, torch.Tensor]:
-        n_local = self.users.shape[0]
+        self._drain()
+        n_local = self._users.shape[0]
         ids = torch.arange(n_local, device=self.cuda_device) * self.world + self.rank
         sel = ids < self.num_users
-        return ids[sel], self.users[sel, : self.k].clone()
+        return ids[sel], self._users[sel, : self.k].clone()
 
     def item_vectors(self) -> Tuple[torch.Tensor, torch.Tensor]:
         """All item vectors of the local shard (the fused kernel does not maintain the touched bitmap:
         with Philox lazy-init every id has a well-defined value whether or not it was pulled)."""
         self.flush()
-        return self.items.dump_local(only_touched=False)
+        return self._items.dump_local(only_touched=False)
 
     # -- checkpoint / resume (the reference only has export + transformWithModelLoad; SURVEY §5) ------
     def save(self, directory: str) -> str:
@@ -343,32 +506,36 @@ class DeviceOnlineMF:
         shard (one-sided assign), replicas are re-pulled."""
         import numpy as np
 
+        self._drain()
         d = np.load(os.path.join(directory, f"rank{self.rank}_of{self.world}.npz"))
         uid = torch.from_numpy(d["user_ids"]).to(self.cuda_device)
-        self.users[uid // self.world, : self.k] = torch.from_numpy(d["user_vecs"]).to(self.cuda_device)
-        self.items.load(torch.from_numpy(d["item_ids"]).to(self.cuda_device),
+        self._users[uid // self.world, : self.k] = torch.from_numpy(d["user_vecs"]).to(self.cuda_device)
+        self._items.load(torch.from_numpy(d["item_ids"]).to(self.cuda_device),
                         torch.from_numpy(d["item_vecs"]).to(self.cuda_device))
         self.step_no = int(d["step_no"])
-        self.items.barrier()
+        self._items.barrier()
         if self.replica is not None:
-            self.replica = ReplicaCache(self.items, self.sync_every, self.sync_interval_ms,
+            self.replica = ReplicaCache(self._items, self.sync_every, self.sync_interval_ms,
                                         require=self.flush_require, flush_count=self.flush_count,
                                         own_inplace=self._own_inplace)
 
     def check_finite(self) -> None:
-        if int(self.nan_flag.item()) != 0:
+        self._drain()
+        if int(self._nan_flag.item()) != 0:
             raise FactorIsNotANumberException("non-finite SGD update")
 
     def barrier(self) -> None:
         self.flush()
-        self.items.barrier()
+        self._items.barrier()
 
     def refresh(self) -> None:
         """Collective quiesce: every delta is in the masters and every replica equals the master."""
+        self._drain()
         if self.replica is not None:
             self.replica.refresh()
         else:
-            self.items.barrier()
+            self._items.barrier()
 
     def close(self) -> None:
-        self.items.close()
+        self._drain()
+        self._items.close()

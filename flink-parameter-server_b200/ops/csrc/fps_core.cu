@@ -194,15 +194,10 @@ __global__ void __launch_bounds__(256, MINB)
     for (int r = 0; r < R; ++r) {
       float d = 0.f;
 #pragma unroll
-      for (int c = 0; c < VPL; ++c)
-        d += u[r][c].x * v[r][c].x + u[r][c].y * v[r][c].y + u[r][c].z * v[r][c].z +
-             u[r][c].w * v[r][c].w;
+      for (int c = 0; c < VPL; ++c) d += fps_mf_dot4(u[r][c], v[r][c]);
       d = fps_group_sum<LPR>(d);
       const float resid = rt[r] - d;
-      const float e = (a.err_mode == 0)   ? 1.f / (1.f + __expf(-resid))
-                      : (a.err_mode == 1) ? resid
-                                          : rt[r] - 1.f / (1.f + __expf(-d));
-      const float g = a.lr * e;
+      const float g = fps_mf_grad(a.err_mode, a.lr, rt[r], d, resid);
       if (LIMIT) {
         __syncwarp();                               // every lane holds its part of the answer
         if ((threadIdx.x & 31) == 0 && ncred[r] > 0) atomicAdd(a.credits, ncred[r]);

@@ -43,3 +43,18 @@ struct MfArgs {
   int* credits;              // device-side pull limiter (WL:196-250): credits[0] = pulls that may still be
                              //   issued, credits[1] = stall counter; nullptr = unlimited
 };
+
+// The pointwise update rule, shared by every fp32 kernel that applies it (fps_core.cu per-launch kernel,
+// fps_mf_window.cu windowed drain): one lane's part of u.v, and the step g = lr * e from the group's dot.
+// Keeping one copy keeps the two paths bitwise equal.  The dot is spelled as the FMA chain nvcc contracts
+// u.x*v.x + u.y*v.y + u.z*v.z + u.w*v.w to (SASS: FMUL y, FFMA x, FFMA z, FFMA w), so that contraction cannot
+// differ between kernels.
+__device__ __forceinline__ float fps_mf_dot4(float4 u, float4 v) {
+  return fmaf(u.w, v.w, fmaf(u.z, v.z, fmaf(u.x, v.x, u.y * v.y)));
+}
+__device__ __forceinline__ float fps_mf_grad(int err_mode, float lr, float rating, float d, float resid) {
+  const float e = (err_mode == 0)   ? 1.f / (1.f + __expf(-resid))
+                  : (err_mode == 1) ? resid
+                                    : rating - 1.f / (1.f + __expf(-d));
+  return lr * e;
+}

@@ -1,0 +1,340 @@
+// Windowed single-GPU MF step: apply a run of staged micro-batches in one item-major pass, so that every
+// item row crosses HBM once per window instead of once per micro-batch.
+//
+// Why: on one GPU the fused per-launch kernel (fps_core.cu) already streams at ~86 % of a copy_, and half of
+// what it moves is item rows: the 1M x 256 B item table is five times the L2, so each micro-batch pulls most of
+// the table from HBM and writes it back.  When the micro-batches of a window are conflict-free -- no user twice
+// in the window, no item twice in a micro-batch -- their result splits into independent per-item chains: for
+// each item, apply its ratings in micro-batch order to a copy of the item row held in registers.  Every user
+// row is read and written by exactly one update, so the arithmetic is the per-launch kernel's, in the same
+// order (same lane geometry, fps_mf_dot4 / fps_mf_grad, adds as add.rn.ftz like red.global.add.f32): the
+// tables come out bitwise equal; only when each row is loaded and stored changes.
+//
+// One cooperative launch per drain (fps_mf_window_kernel), looping until every staged micro-batch is applied:
+//   1. build: clear the user bitmap; scatter micro-batch start, start+1, ... (one per grid sync) into the
+//      item-major slot table T[j - start][item] = {user slot, rating} with atomicExch, test-and-setting each
+//      user's bit.  An occupied T entry or an already-set bit is a conflict: the window ends before that
+//      micro-batch.
+//   2. chain: one lane-group per item reads its entries, pulls the item row once and the chain's user rows
+//      together, applies the updates in order, stores each row once and resets every T entry it saw.
+//   3. singleton: a micro-batch that conflicts with itself (an item or a user twice in it) is applied alone
+//      with the per-launch update (pull both rows, red.global.add both deltas): racy as it is today.
+#include <cuda_fp16.h>
+#include <cooperative_groups.h>
+#include "fps_common.cuh"
+#include "fps_mf_args.cuh"
+
+namespace cg = cooperative_groups;
+
+#define WIN_MAX 8            // micro-batches per window (T rows)
+#define WIN_THREADS 256
+#define WIN_EMPTY 0xFFFFFFFFFFFFFFFFull
+
+struct WinArgs {
+  const unsigned char* stage;   // staged records, slot j at stage + j * slot_bytes
+  long long slot_bytes;
+  long long n[WIN_MAX];         // records per slot
+  int fmt[WIN_MAX];             // 0: int32 users[n] | int32 items[n] | fp32 ratings[n];  1: packed64[n]
+  int n_slots;
+  int err_mode;
+  float lr;
+  int stride;                   // row stride in floats (user and item tables)
+  float* user_table;            // [n_local, stride], slot = user (one worker)
+  float* item_table;            // [rows, stride]
+  long long rows;               // item rows = T row length
+  unsigned long long* slots;    // T [n_slots, rows]; WIN_EMPTY everywhere between drains
+  unsigned int* user_bits;      // [bm_words]
+  long long bm_words;
+  unsigned int* ctl;            // [2 * WIN_MAX] conflict flag per scatter attempt (zeroed by the kernel)
+  float* stats;                 // [2] += window totals
+  float* slot_stats;            // [n_slots, 2] per-micro-batch (sum sq err, updates) (zeroed by the kernel)
+  int* nan_flag;
+};
+
+__device__ __forceinline__ bool win_record(const WinArgs& a, int j, long long i, int& user, int& item,
+                                           float& rating) {
+  const unsigned char* base = a.stage + (long long)j * a.slot_bytes;
+  if (a.fmt[j] == 1) {
+    const unsigned long long rec = reinterpret_cast<const unsigned long long*>(base)[i];
+    user = (int)(rec >> 38);
+    item = (int)((rec >> 16) & 0x3FFFFFull);
+    rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
+    return true;
+  }
+  const long long n = a.n[j];
+  user = reinterpret_cast<const int*>(base)[i];
+  item = reinterpret_cast<const int*>(base)[n + i];
+  rating = reinterpret_cast<const float*>(base)[2 * n + i];
+  return user >= 0;   // record voided upstream
+}
+
+__device__ __forceinline__ float win_add(float x, float y) {
+  float z;
+  asm("add.rn.ftz.f32 %0, %1, %2;" : "=f"(z) : "f"(x), "f"(y));
+  return z;
+}
+__device__ __forceinline__ float4 win_add4(float4 x, float g, float4 y) {   // x + g * y, rounded like the REDG
+  return make_float4(win_add(x.x, g * y.x), win_add(x.y, g * y.y), win_add(x.z, g * y.z), win_add(x.w, g * y.w));
+}
+
+// Per-slot (sum sq err, updates) sums: slot r lives in lane r % LPR of every lane-group, at index r / LPR.
+// Flushed as warp sums -> CTA sums in shared memory -> one atomic per (CTA, slot) into slot_stats[slot0 + r].
+template <int LPR, int NS>
+__device__ __forceinline__ void win_flush_stats(const WinArgs& a, float (&sq)[NS], float (&cnt)[NS], int nr,
+                                                int slot0, float* sh) {
+  const int lane = threadIdx.x & (LPR - 1);
+  __syncthreads();
+  if (threadIdx.x < 2 * WIN_MAX) sh[threadIdx.x] = 0.f;
+  __syncthreads();
+#pragma unroll
+  for (int r = 0; r < WIN_MAX; ++r) {
+    if (r < nr) {
+      const bool mine = lane == r % LPR;
+      float s = mine ? sq[r / LPR] : 0.f, c = mine ? cnt[r / LPR] : 0.f;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        s += __shfl_xor_sync(0xffffffffu, s, o);
+        c += __shfl_xor_sync(0xffffffffu, c, o);
+      }
+      if ((threadIdx.x & 31) == 0 && c > 0.f) {
+        atomicAdd(sh + 2 * r, s);
+        atomicAdd(sh + 2 * r + 1, c);
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < NS; ++i) sq[i] = cnt[i] = 0.f;
+  __syncthreads();
+  if (threadIdx.x < 2 * nr && sh[threadIdx.x] != 0.f)
+    atomicAdd(a.slot_stats + 2 * slot0 + threadIdx.x, sh[threadIdx.x]);
+}
+
+// LPR lanes per row, one float4 per lane (the dispatch_mf geometry for rows of up to 32 float4); P = user rows
+// prefetched together per lane-group, MINB = CTAs per SM the registers are held to.
+template <int LPR, int P, int MINB>
+__global__ void __launch_bounds__(WIN_THREADS, MINB) fps_mf_window_kernel(const __grid_constant__ WinArgs a) {
+  __shared__ float sh[2 * WIN_MAX];
+  cg::grid_group grid = cg::this_grid();
+  const int lane = threadIdx.x & (LPR - 1);
+  const long long gtid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  const long long gthreads = (long long)gridDim.x * blockDim.x;
+  const long long group = gtid / LPR;
+  const long long n_groups = gthreads / LPR;
+  const int stride = a.stride;
+  const bool col = lane < (stride >> 2);   // this lane owns a float4 of the row
+  constexpr int NS = LPR < WIN_MAX ? WIN_MAX / LPR : 1;
+  constexpr int NE = NS;   // T entries per lane in the chain
+  float sq[NS], cnt[NS];   // see win_flush_stats
+#pragma unroll
+  for (int i = 0; i < NS; ++i) sq[i] = cnt[i] = 0.f;
+  bool bad = false;
+
+  if (blockIdx.x == 0) {
+    if (threadIdx.x < 2 * WIN_MAX) a.ctl[threadIdx.x] = 0u;
+    if (threadIdx.x < 2 * a.n_slots) a.slot_stats[threadIdx.x] = 0.f;
+  }
+  int start = 0, attempt = 0;
+  while (start < a.n_slots) {
+    // ---- 1. build -------------------------------------------------------------------------------------
+    for (long long w = gtid; w < a.bm_words; w += gthreads) a.user_bits[w] = 0u;
+    grid.sync();
+    int end = start;
+    bool clashed = false;
+    while (end < a.n_slots) {
+      const int j = end;
+      unsigned long long* t = a.slots + (long long)(j - start) * a.rows;
+      bool clash = false;
+      for (long long i = gtid; i < a.n[j]; i += gthreads) {
+        int user, item;
+        float rating;
+        if (!win_record(a, j, i, user, item, rating)) continue;
+        const unsigned long long e = ((unsigned long long)__float_as_uint(rating) << 32) | (unsigned int)user;
+        clash |= atomicExch(t + item, e) != WIN_EMPTY;
+        const unsigned int bit = 1u << (user & 31);
+        clash |= (atomicOr(a.user_bits + (user >> 5), bit) & bit) != 0u;
+      }
+      if (clash) *reinterpret_cast<volatile unsigned int*>(a.ctl + attempt) = 1u;
+      grid.sync();
+      clashed = *reinterpret_cast<volatile unsigned int*>(a.ctl + attempt) != 0u;
+      ++attempt;
+      if (clashed) break;
+      ++end;
+    }
+    const int nrow = end - start;                  // micro-batches in the window
+    const int written = nrow + (clashed ? 1 : 0);  // T rows holding entries (the clashing one partially)
+    if (nrow > 0) {
+      // ---- 2. chain -------------------------------------------------------------------------------------
+      // T entries: lane l of the group loads rows r = l, l + LPR, ... of its item (every T entry the window
+      // wrote, the clashing micro-batch's partial row included), one item ahead of the chain, and resets
+      // them itself; the chain gets them by shuffles.
+      unsigned long long nxt[NE];
+#pragma unroll
+      for (int m = 0; m < NE; ++m) {
+        const int r = lane + m * LPR;
+        nxt[m] = (group < a.rows && r < written) ? a.slots[(long long)r * a.rows + group] : WIN_EMPTY;
+      }
+      for (long long base = 0; base < a.rows; base += n_groups) {   // warp-uniform trip count
+        const long long item = base + group;
+        const bool in = item < a.rows;
+        float* vp = a.item_table + (in ? item : 0) * (long long)stride + 4 * lane;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        bool any = false;
+        bool loaded = false;
+        unsigned long long mine[NE];
+#pragma unroll
+        for (int m = 0; m < NE; ++m) {
+          const int r = lane + m * LPR;
+          mine[m] = nxt[m];
+          const long long it2 = item + n_groups;
+          nxt[m] = (it2 < a.rows && r < written) ? a.slots[(long long)r * a.rows + it2] : WIN_EMPTY;
+          if (mine[m] != WIN_EMPTY) a.slots[(long long)r * a.rows + item] = WIN_EMPTY;
+        }
+        const int src0 = (threadIdx.x & 31) & ~(LPR - 1);   // the group's first lane in the warp
+#pragma unroll
+        for (int c0 = 0; c0 < WIN_MAX; c0 += P) {
+          if (c0 < nrow) {
+            unsigned long long ent[P];
+#pragma unroll
+            for (int q = 0; q < P; ++q) {
+              const int r = c0 + q;
+              ent[q] = __shfl_sync(0xffffffffu, mine[(r / LPR) % NE], src0 + r % LPR);
+              if (r >= nrow) ent[q] = WIN_EMPTY;   // the clashing micro-batch is not applied
+            }
+            {
+              bool chunk_any = false;
+#pragma unroll
+              for (int q = 0; q < P; ++q) chunk_any |= ent[q] != WIN_EMPTY;
+              if (chunk_any && !loaded && col) v = *reinterpret_cast<const float4*>(vp);
+              loaded |= chunk_any;
+              any |= chunk_any;
+              float4 u[P];
+#pragma unroll
+              for (int q = 0; q < P; ++q) {
+                const float* up = a.user_table + (long long)(unsigned int)ent[q] * stride + 4 * lane;
+                u[q] = (ent[q] != WIN_EMPTY && col) ? *reinterpret_cast<const float4*>(up)
+                                                    : make_float4(0.f, 0.f, 0.f, 0.f);
+              }
+#pragma unroll
+              for (int q = 0; q < P; ++q) {
+                const int r = c0 + q;
+                if (r < nrow) {                    // grid-uniform: the group sum sees the whole warp
+                  float d = 0.f;
+                  d += fps_mf_dot4(u[q], v);
+                  d = fps_group_sum<LPR>(d);
+                  const bool ok = ent[q] != WIN_EMPTY;
+                  const float rating = __uint_as_float((unsigned int)(ent[q] >> 32));
+                  const float resid = rating - d;
+                  const float g = fps_mf_grad(a.err_mode, a.lr, rating, d, resid);
+                  if (ok) {
+                    if (!(fabsf(g) <= 3.0e38f)) bad = true;  // NaN/Inf guard, as the per-launch kernel
+                    if (lane == r % LPR) {
+                      sq[r / LPR] += resid * resid;
+                      cnt[r / LPR] += 1.f;
+                    }
+                    const float4 nu = win_add4(u[q], g, v);
+                    v = win_add4(v, g, u[q]);
+                    if (col)
+                      *reinterpret_cast<float4*>(a.user_table + (long long)(unsigned int)ent[q] * stride +
+                                                 4 * lane) = nu;
+                  }
+                }
+              }
+            }
+          }
+        }
+        if (any && col) *reinterpret_cast<float4*>(vp) = v;
+      }
+      win_flush_stats<LPR, NS>(a, sq, cnt, nrow, start, sh);
+    } else {
+      // ---- 3. singleton: micro-batch `start` has an item or a user twice ----------------------------------
+      const int j = start;
+      unsigned long long* t = a.slots;
+      for (long long base = 0; base < a.n[j]; base += n_groups) {
+        const long long i = base + group;
+        int user = 0, item = 0;
+        float rating = 0.f;
+        const bool ok = i < a.n[j] && win_record(a, j, i, user, item, rating);
+        float* up = a.user_table + (long long)user * stride + 4 * lane;
+        float* vp = a.item_table + (long long)item * stride + 4 * lane;
+        float4 u = make_float4(0.f, 0.f, 0.f, 0.f), v = u;
+        if (ok && col) {
+          v = fps_ld_row4(vp);
+          u = *reinterpret_cast<const float4*>(up);
+        }
+        float d = 0.f;
+        d += fps_mf_dot4(u, v);
+        d = fps_group_sum<LPR>(d);
+        const float resid = rating - d;
+        const float g = fps_mf_grad(a.err_mode, a.lr, rating, d, resid);
+        if (ok) {
+          if (!(fabsf(g) <= 3.0e38f)) bad = true;
+          if (lane == 0) {
+            sq[0] += resid * resid;
+            cnt[0] += 1.f;
+            t[item] = WIN_EMPTY;
+          }
+          if (col) {
+            fps_red_add4(up, make_float4(g * v.x, g * v.y, g * v.z, g * v.w));
+            fps_red_add4(vp, make_float4(g * u.x, g * u.y, g * u.z, g * u.w));
+          }
+        }
+      }
+      win_flush_stats<LPR, NS>(a, sq, cnt, 1, start, sh);
+      end = start + 1;
+    }
+    grid.sync();
+    start = end;
+  }
+  if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
+  if (blockIdx.x == 0 && threadIdx.x == 0 && a.stats != nullptr) {
+    float s = 0.f, c = 0.f;
+    for (int j = 0; j < a.n_slots; ++j) {
+      s += a.slot_stats[2 * j];
+      c += a.slot_stats[2 * j + 1];
+    }
+    a.stats[0] += s;
+    a.stats[1] += c;
+  }
+}
+
+template <int LPR, int P, int MINB>
+static int launch_window(const WinArgs& a, int num_sms, cudaStream_t stream) {
+  int occ = 0;
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fps_mf_window_kernel<LPR, P, MINB>, WIN_THREADS, 0);
+  if (e != cudaSuccess) return (int)e;
+  if (occ < 1) return -1402;
+  const long long grid = (long long)num_sms * occ;   // every CTA resident (grid sync)
+  WinArgs args = a;
+  void* params[] = {&args};
+  e = cudaLaunchCooperativeKernel((const void*)fps_mf_window_kernel<LPR, P, MINB>, dim3((unsigned)grid),
+                                  dim3(WIN_THREADS), params, 0, stream);
+  if (e != cudaSuccess) return (int)e;
+  return (int)cudaGetLastError();
+}
+
+static int g_win_variant = 0;  // tuning knob: (user rows prefetched, CTAs/SM), see dispatch_window
+extern "C" void fps_set_mf_window_variant(int v) { g_win_variant = v; }
+
+template <int LPR>
+static int dispatch_window(const WinArgs& a, int num_sms, cudaStream_t s) {
+  switch (g_win_variant) {
+    case 1: return launch_window<LPR, 8, 1>(a, num_sms, s);   // all 8 user rows of a chain at once, 2 CTAs/SM
+    default:
+      if constexpr (LPR <= 2) return launch_window<LPR, 4, 2>(a, num_sms, s);   // more per-slot sums per lane
+      else return launch_window<LPR, 4, 3>(a, num_sms, s);
+  }
+}
+
+// Rows of up to 32 float4 (k <= 128): the geometry dispatch_mf picks for them (one float4 per lane).
+extern "C" int fps_mf_window_drain(const WinArgs* a, int num_sms, cudaStream_t stream) {
+  if (a->n_slots <= 0) return 0;
+  if (a->n_slots > WIN_MAX) return -1401;
+  const int nvec = a->stride >> 2;
+  if (nvec <= 1) return dispatch_window<1>(*a, num_sms, stream);
+  if (nvec <= 2) return dispatch_window<2>(*a, num_sms, stream);
+  if (nvec <= 4) return dispatch_window<4>(*a, num_sms, stream);
+  if (nvec <= 8) return dispatch_window<8>(*a, num_sms, stream);
+  if (nvec <= 16) return dispatch_window<16>(*a, num_sms, stream);
+  if (nvec <= 32) return dispatch_window<32>(*a, num_sms, stream);
+  return -1400;
+}

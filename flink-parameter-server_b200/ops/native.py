@@ -312,6 +312,62 @@ def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
     _bump()
 
 
+WINDOW_MAX = 8   # micro-batches per drain (csrc/fps_mf_window.cu WIN_MAX)
+
+
+class WinArgsC(C.Structure):
+    """Mirror of ``struct WinArgs`` (csrc/fps_mf_window.cu)."""
+
+    _fields_ = [
+        ("stage", C.c_void_p), ("slot_bytes", C.c_longlong),
+        ("n", C.c_longlong * WINDOW_MAX), ("fmt", C.c_int * WINDOW_MAX),
+        ("n_slots", C.c_int), ("err_mode", C.c_int), ("lr", C.c_float), ("stride", C.c_int),
+        ("user_table", C.c_void_p), ("item_table", C.c_void_p), ("rows", C.c_longlong),
+        ("slots", C.c_void_p), ("user_bits", C.c_void_p), ("bm_words", C.c_longlong),
+        ("ctl", C.c_void_p), ("stats", C.c_void_p), ("slot_stats", C.c_void_p), ("nan_flag", C.c_void_p),
+    ]
+
+
+def mf_window_drain(stage: torch.Tensor, slot_bytes: int, counts, formats, user_table: torch.Tensor,
+                    item_table: torch.Tensor, lr: float, err_mode: int, slots: torch.Tensor,
+                    user_bits: torch.Tensor, ctl: torch.Tensor, stats: torch.Tensor, slot_stats: torch.Tensor,
+                    nan_flag: torch.Tensor) -> None:
+    """Apply the micro-batches staged in ``stage`` (slot j at byte ``j * slot_bytes``: ``counts[j]`` records,
+    ``formats[j]`` 1 = packed64, 0 = int32 users | int32 items | fp32 ratings) in order, in one cooperative
+    launch (csrc/fps_mf_window.cu).  Conflict-free runs of micro-batches are applied item-major with the tables
+    bitwise equal to one :func:`mf_sgd_fused` launch per micro-batch.  ``slots``: int64 ``[>= n, rows]``
+    filled with -1, left so; ``user_bits``: int32 bitmap over the user rows; ``ctl``: int32 ``[2 * WINDOW_MAX]``;
+    ``slot_stats``: float32 ``[>= n, 2]`` receives each micro-batch's (sum sq err, updates), ``stats`` the totals
+    (``DeviceOnlineMF`` reads only the totals; the per-micro-batch sums serve callers that report per micro-batch)."""
+    n = len(counts)
+    if not 0 < n <= WINDOW_MAX or len(formats) != n:
+        raise ValueError(f"1..{WINDOW_MAX} staged micro-batches expected, got {n}")
+    for t, name in ((stage, "stage"), (user_table, "user_table"), (item_table, "item_table"), (slots, "slots"),
+                    (user_bits, "user_bits"), (ctl, "ctl"), (stats, "stats"), (slot_stats, "slot_stats"),
+                    (nan_flag, "nan_flag")):
+        _req(t, name)
+    if user_table.shape[1] != item_table.shape[1]:
+        raise ValueError("user table stride must equal item table stride")
+    if user_bits.numel() * 32 < user_table.shape[0] or slots.numel() < n * item_table.shape[0]:
+        raise ValueError("user bitmap or slot table too small")
+    if slot_stats.numel() < 2 * n or ctl.numel() < 2 * WINDOW_MAX:
+        raise ValueError("slot_stats / ctl too small")
+    a = WinArgsC()
+    a.stage = stage.data_ptr(); a.slot_bytes = int(slot_bytes)
+    for j in range(n):
+        a.n[j] = int(counts[j]); a.fmt[j] = int(formats[j])
+    a.n_slots = n; a.err_mode = int(err_mode); a.lr = float(lr); a.stride = int(item_table.shape[1])
+    a.user_table = user_table.data_ptr(); a.item_table = item_table.data_ptr(); a.rows = int(item_table.shape[0])
+    a.slots = slots.data_ptr(); a.user_bits = user_bits.data_ptr(); a.bm_words = user_bits.numel()
+    a.ctl = ctl.data_ptr(); a.stats = stats.data_ptr(); a.slot_stats = slot_stats.data_ptr()
+    a.nan_flag = nan_flag.data_ptr()
+    rv = os.environ.get("FPS_MF_WINDOW_VARIANT")
+    if rv is not None:
+        lib().fps_set_mf_window_variant(int(rv))
+    _check(lib().fps_mf_window_drain(C.byref(a), sm_count(stage.device.index), _stream()), "mf_window_drain")
+    _bump()
+
+
 class BprArgsC(C.Structure):
     """Mirror of ``struct BprArgs`` (csrc/fps_mf_bpr.cu)."""
 
