@@ -199,11 +199,24 @@ def bpr_delta(u: Vector, vi: Vector, vj: Vector, lr: float, reg: float):
     return du, dvi, dvj, loss
 
 
+def rowwise_adagrad(row: Vector, G: float, delta: Vector, lr: float, k: int, eps: float = 1e-8):
+    """One row-wise AdaGrad step of a row whose learning-rate-1 SGD delta is ``delta`` and whose accumulator
+    reads ``G``: ``s = |delta|^2 / k``, ``row + lr * delta / (sqrt(G + s) + eps)``.  Returns ``(new_row, s)``; the
+    accumulator becomes ``G + s``.  ``k`` is the logical factor count.  The reference of the device kernels'
+    ``optimizer="adagrad"``."""
+    delta = np.asarray(delta, dtype=np.float64)
+    s = float(np.dot(delta, delta)) / k
+    return np.asarray(row, dtype=np.float64) + lr * delta / (math.sqrt(G + s) + eps), s
+
+
 def require_pointwise(backend: str, kw: dict) -> None:
-    """The host tiers (``backend="local"`` / ``"native"``) train the pointwise loss only."""
+    """The host tiers (``backend="local"`` / ``"native"``) train the pointwise loss with SGD only."""
     if backend != "device" and (kw.get("loss", "pointwise") != "pointwise" or kw.get("regularization", 0)):
         raise ValueError(f"loss={kw.get('loss')!r} / regularization need backend='device' "
                          f"(backend={backend!r} trains the pointwise loss only)")
+    if backend != "device" and kw.get("optimizer", "sgd") != "sgd":
+        raise ValueError(f"optimizer={kw.get('optimizer')!r} needs backend='device' "
+                         f"(backend={backend!r} trains with SGD only)")
 
 
 # ---- top-K ------------------------------------------------------------------------------

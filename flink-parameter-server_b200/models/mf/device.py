@@ -40,16 +40,37 @@ WINDOW_BYTES_PER_ROW = 8 + 12  # per item row and window slot: one slot-table en
 WINDOW_MAX_STRIDE = 128        # floats per row the window kernel handles (k <= 128)
 
 
+OPTIMIZERS = ("sgd", "adagrad")
+
+
+def check_optimizer(optimizer: str, *, item_cache: bool, output_ring=None, kernel: Optional[str] = None) -> None:
+    """Raise ``ValueError`` for an optimizer :class:`DeviceOnlineMF` cannot run with these settings.  Row-wise
+    AdaGrad runs per launch on the register-staged kernel, reading its accumulators where the rows live, so it
+    needs the direct mode (``item_cache=False``) and has no output ring or TMA kernel."""
+    if optimizer not in OPTIMIZERS:
+        raise ValueError(f"optimizer must be 'sgd' or 'adagrad', got {optimizer!r}")
+    if optimizer == "sgd":
+        return
+    if item_cache:
+        raise ValueError("optimizer='adagrad' is not supported in the replica (item_cache) mode, the multi-GPU "
+                         "default: pass item_cache=False to read and update the item rows on their owners")
+    if output_ring is not None:
+        raise ValueError("optimizer='adagrad' does not support the per-update output ring (output_ring=None)")
+    if kernel == "tma":
+        raise ValueError("optimizer='adagrad' runs on the register-staged kernel: pass kernel=None or 'reg'")
+
+
 def step_window_size(step_window: Optional[int], *, world: int, item_cache: bool, loss: str, table_rows: int,
-                     stride: int, env: Optional[str] = None) -> int:
+                     stride: int, env: Optional[str] = None, optimizer: str = "sgd") -> int:
     """Micro-batches per step window of :class:`DeviceOnlineMF` (0 = off).
 
     ``None`` = auto: on for one worker without an item cache whose item table exceeds the L2 (where every
     micro-batch re-reads it from HBM), unless ``FPS_STEP_WINDOW=0`` (``env``).  ``0`` / ``1`` = off, ``n >= 2`` =
     at most ``n`` (and at most ``native.WINDOW_MAX``).  The slot table and the staging area take
     ``W * table_rows * 20`` bytes, capped at ``WINDOW_BUDGET``: ``W`` is lowered to fit, and the window is off
-    below 2."""
-    if world != 1 or item_cache or loss != "pointwise" or stride > WINDOW_MAX_STRIDE or table_rows < 1:
+    below 2.  Row-wise AdaGrad (``optimizer="adagrad"``) runs per launch: 0."""
+    if world != 1 or item_cache or loss != "pointwise" or optimizer != "sgd" or stride > WINDOW_MAX_STRIDE \
+            or table_rows < 1:
         return 0
     if step_window is None:
         if env == "0" or table_rows * stride * 4 <= L2_TABLE_BYTES:
@@ -87,13 +108,18 @@ class DeviceOnlineMF:
                  block_bytes: int = 16 << 20, flush_count: Optional[int] = None,
                  flush_require: str = "any", replica_own_inplace: Optional[bool] = None,
                  output_ring=None, loss: str = "pointwise", regularization: float = 0.0,
-                 step_window: Optional[int] = None):
+                 step_window: Optional[int] = None, optimizer: str = "sgd"):
         """``loss="bpr"``: pairwise (Bayesian Personalised Ranking) updates, each positive rating paired
         with ``negative_sample_rate`` negatives (sampled) or with the ``negatives=`` of :meth:`step`;
         ``regularization`` is its L2 weight.  The pointwise loss has no regulariser.
 
         ``step_window``: how many micro-batches :meth:`step` may defer and then apply in one item-major pass
-        (see :meth:`step` and :func:`step_window_size`; ``None`` = auto, ``0`` = off)."""
+        (see :meth:`step` and :func:`step_window_size`; ``None`` = auto, ``0`` = off).
+
+        ``optimizer="adagrad"``: row-wise AdaGrad (DESIGN §2.10) instead of SGD with one global rate.  Each row
+        keeps one fp32 accumulator ``G`` of its mean squared delta and steps by ``learning_rate / (sqrt(G) +
+        1e-8)``; users' accumulators stay on their worker, items' on the item's shard.  It runs per launch (no
+        step window) in the direct mode only: ``item_cache=False`` when there is more than one GPU."""
         self._pending = []           # staged micro-batches of the step window: (records, format)
         self.step_window = 0
         if loss not in ("pointwise", "bpr"):
@@ -115,6 +141,10 @@ class DeviceOnlineMF:
         ready = dist.is_available() and dist.is_initialized()
         self.world = dist.get_world_size(group) if ready else 1
         self.rank = dist.get_rank(group) if ready else 0
+        if item_cache is None:
+            item_cache = self.world > 1 and os.environ.get("FPS_ITEM_CACHE", "1") != "0"
+        check_optimizer(optimizer, item_cache=bool(item_cache), output_ring=output_ring, kernel=kernel)
+        self.optimizer = optimizer
         self.num_users, self.num_items, self.k = int(num_users), int(num_items), int(num_factors)
         self.lr = float(learning_rate)
         self.neg = int(negative_sample_rate)
@@ -129,7 +159,7 @@ class DeviceOnlineMF:
         # (the BPR kernel has only the static form)
         self.credits = (torch.tensor([self.pull_limit, 0], dtype=torch.int32, device=self.cuda_device)
                         if self.pull_limit >= 32 and os.environ.get("FPS_STATIC_LIMITER", "0") != "1"
-                        and loss == "pointwise" else None)
+                        and loss == "pointwise" and optimizer == "sgd" else None)
         self.output_ring = output_ring     # E5: per-update (user, vector) output stream (runtime/output_ring.py)
         with torch.cuda.device(self.device):
             # parameter server: item vectors, sharded item % psParallelism
@@ -145,6 +175,11 @@ class DeviceOnlineMF:
                              seed * 2 + 2, range_min, range_max)
             # pointwise: [sum (r - u.v)^2, updates]; BPR: [sum softplus(-x), triples, triples with x > 0]
             self._stats = torch.zeros(3 if loss == "bpr" else 2, dtype=torch.float32, device=self.cuda_device)
+            # row-wise AdaGrad: one fp32 accumulator per user row (worker-local) and per item row (item shard)
+            self._user_acc = self._item_acc = None
+            if optimizer == "adagrad":
+                self._user_acc = torch.zeros(n_local, dtype=torch.float32, device=self.cuda_device)
+                self._item_acc = self._items.row_accumulators()
             self._nan_flag = torch.zeros(1, dtype=torch.int32, device=self.cuda_device)
             # K5: per-user memory of recently seen items (userMemory of the reference, default 128
             # there; 0 here = sample uniformly inside the fused kernel, rejecting only the positive)
@@ -161,8 +196,6 @@ class DeviceOnlineMF:
         # staggered -- and a few TMA-driven CTAs (fps_replica_exchange) push (replica - base) to those
         # master shards and fold the other workers' contributions (master - base) into the replica while
         # the training kernel keeps running.  Asynchronous (no barriers); staleness ~ `sync_every` steps.
-        if item_cache is None:
-            item_cache = self.world > 1 and os.environ.get("FPS_ITEM_CACHE", "1") != "0"
         self.item_cache = bool(item_cache)
         self.sync_every = max(1, int(sync_every))
         self.sync_interval_ms = sync_interval_ms
@@ -198,7 +231,7 @@ class DeviceOnlineMF:
         # ---- step window (fps_mf_window.cu): buffers allocated by the first windowed step ----------------
         self.step_window = step_window_size(step_window, world=self.world, item_cache=self.item_cache,
                                             loss=self.loss, table_rows=self.num_items, stride=self._items.stride,
-                                            env=os.environ.get("FPS_STEP_WINDOW"))
+                                            env=os.environ.get("FPS_STEP_WINDOW"), optimizer=optimizer)
         self._win = None
         self._graph_capture = False
         self._per_launch = False
@@ -224,6 +257,15 @@ class DeviceOnlineMF:
     def nan_flag(self) -> torch.Tensor:
         self._drain()
         return self._nan_flag
+
+    @property
+    def accumulators(self) -> Optional[Tuple[torch.Tensor, torch.Tensor]]:
+        """Row-wise AdaGrad state ``(user_acc [n_local], item_acc_local [rows_per_shard])``, slot-indexed like
+        ``users`` and ``items.local``; ``None`` with ``optimizer="sgd"``."""
+        self._drain()
+        if self._item_acc is None:
+            return None
+        return self._user_acc, self._item_acc.local
 
     def _windowable(self, users, items, ratings) -> bool:
         if self.step_window < 2 or self._graph_capture or self._per_launch:
@@ -354,7 +396,9 @@ class DeviceOnlineMF:
                                 num_items=self.num_items, seed=self.seed, step=self.step_no,
                                 stats=self._stats, nan_flag=self._nan_flag,
                                 max_inflight_rows=self.pull_limit, kernel=self.kernel,
-                                l2_hints=self.l2_hints, output=out_args, credits=self.credits)
+                                l2_hints=self.l2_hints, output=out_args, credits=self.credits,
+                                item_acc=self._item_acc.table_c if self._item_acc is not None else None,
+                                user_acc=self._user_acc)
         if ring is not None:               # device-side count / timer policy + flush to the pinned host ring
             ring.after_kernel(users.numel() * (1 + neg))
         self.step_no += 1
@@ -390,7 +434,9 @@ class DeviceOnlineMF:
         native.mf_bpr_fused(users, items, ratings, self._users, cand, self.lr, self.reg, negatives=negatives,
                             n_neg=n, num_items=self.num_items, seed=self.seed, step=self.step_no,
                             anchor_div=self.world, stats=self._stats, nan_flag=self._nan_flag,
-                            max_inflight_rows=self.pull_limit, reserve_total=reserve)
+                            max_inflight_rows=self.pull_limit, reserve_total=reserve,
+                            anchor_acc=self._user_acc,
+                            cand_acc=self._item_acc.table_c if self._item_acc is not None else None)
         self.step_no += 1
         METRICS.inc("mf_ratings", n_pos)
 
@@ -489,7 +535,8 @@ class DeviceOnlineMF:
 
     # -- checkpoint / resume (the reference only has export + transformWithModelLoad; SURVEY §5) ------
     def save(self, directory: str) -> str:
-        """Every rank writes its user partition and its item shard to ``directory/rank<r>.npz``."""
+        """Every rank writes its user partition and its item shard to ``directory/rank<r>.npz``, with their
+        AdaGrad accumulators when ``optimizer="adagrad"``."""
         import numpy as np
 
         os.makedirs(directory, exist_ok=True)
@@ -497,13 +544,19 @@ class DeviceOnlineMF:
         uid, uvec = self.user_vectors()
         iid, ivec = self.item_vectors()
         path = os.path.join(directory, f"rank{self.rank}_of{self.world}.npz")
+        extra = {}
+        if self._item_acc is not None:
+            aid, aval = self._item_acc.dump_local()
+            extra = dict(user_acc=self._user_acc[uid // self.world].cpu().numpy(), item_acc_ids=aid.cpu().numpy(),
+                         item_acc=aval.cpu().numpy())
         np.savez(path, user_ids=uid.cpu().numpy(), user_vecs=uvec.cpu().numpy(), item_ids=iid.cpu().numpy(),
-                 item_vecs=ivec.cpu().numpy(), step_no=self.step_no)
+                 item_vecs=ivec.cpu().numpy(), step_no=self.step_no, **extra)
         return path
 
     def load(self, directory: str) -> None:
         """Resume from :meth:`save` (same world size): users go back to their worker, items to their
-        shard (one-sided assign), replicas are re-pulled."""
+        shard (one-sided assign), replicas are re-pulled.  AdaGrad accumulators are restored, or zeroed when
+        the checkpoint has none."""
         import numpy as np
 
         self._drain()
@@ -513,6 +566,13 @@ class DeviceOnlineMF:
         self._items.load(torch.from_numpy(d["item_ids"]).to(self.cuda_device),
                         torch.from_numpy(d["item_vecs"]).to(self.cuda_device))
         self.step_no = int(d["step_no"])
+        if self._item_acc is not None:
+            self._user_acc.zero_()
+            self._item_acc.local.zero_()
+            if "item_acc" in d.files:
+                self._user_acc[uid // self.world] = torch.from_numpy(d["user_acc"]).to(self.cuda_device)
+                self._item_acc.load(torch.from_numpy(d["item_acc_ids"]).to(self.cuda_device),
+                                    torch.from_numpy(d["item_acc"]))
         self._items.barrier()
         if self.replica is not None:
             self.replica = ReplicaCache(self._items, self.sync_every, self.sync_interval_ms,
@@ -538,4 +598,6 @@ class DeviceOnlineMF:
 
     def close(self) -> None:
         self._drain()
+        if self._item_acc is not None:
+            self._item_acc.close()
         self._items.close()

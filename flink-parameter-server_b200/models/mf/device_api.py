@@ -73,13 +73,16 @@ def ps_online_mf_device(src, numFactors=10, rangeMin=-0.01, rangeMax=0.01, learn
                         batch_size: int = 1 << 16, group=None, epochs: int = 1,
                         userMemory: int = 128, updateOutput: Optional[int] = None,
                         outputFlushCount: int = 1, outputFlushMs: Optional[float] = None,
-                        loss: str = "pointwise", regularization: float = 0.0) -> ResultStream:
+                        loss: str = "pointwise", regularization: float = 0.0,
+                        optimizer: str = "sgd") -> ResultStream:
     """``updateOutput=n``: also emit ``Left((userId, userVector))`` for one update in ``n`` (``1`` = every
     update, the reference's worker output PSOnlineMatrixFactorizationWorker.scala:52) through the device
     output ring (count / timer flushed on the device); the final dump then holds only the item shard.
     ``loss="bpr"``: pairwise updates, every rating > 0 paired with ``negativeSampleRate`` sampled
     negatives, L2 weight ``regularization`` (see :class:`DeviceOnlineMF`); it has no per-update output,
-    so ``updateOutput`` with ``loss="bpr"`` raises ``ValueError``."""
+    so ``updateOutput`` with ``loss="bpr"`` raises ``ValueError``.
+    ``optimizer="adagrad"``: row-wise AdaGrad (see :class:`DeviceOnlineMF`); a multi-rank job then reads and
+    updates the item rows on their owners (no item cache)."""
     if updateOutput and loss != "pointwise":
         raise ValueError("updateOutput (the per-update output ring) is not supported with loss='bpr'")
     recs = None
@@ -97,7 +100,8 @@ def ps_online_mf_device(src, numFactors=10, rangeMin=-0.01, rangeMax=0.01, learn
                            group=group, seed=seed, err_mode=ERR_PLAIN if plain_residual else ERR_SIGMOID,
                            track_touched=True,
                            user_memory=min(int(userMemory), 256) if negativeSampleRate > 0 else 0,
-                           loss=loss, regularization=regularization)
+                           loss=loss, regularization=regularization, optimizer=optimizer,
+                           item_cache=False if optimizer == "adagrad" else None)
     ring, updates = None, []
     if updateOutput:
         from ...runtime.output_ring import OutputRing

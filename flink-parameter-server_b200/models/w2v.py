@@ -8,6 +8,8 @@ from their owners, and pushes ``g*v`` to ``W_in[center]`` and ``g*u`` to ``W_out
 ``red.global.add.v4.f32`` -- the additive paramUpdate happens in the owner's memory system.
 ``negative`` extra pairs per positive are sampled on the device (uniform over the vocabulary) with
 label 0.  Not part of the reference's algorithm suite; it exercises the same API on a 1.2 KB row.
+``optimizer="adagrad"`` replaces the global rate by row-wise AdaGrad (DESIGN §2.10), with one fp32
+accumulator per row of each table on that row's shard.
 """
 from __future__ import annotations
 
@@ -27,7 +29,15 @@ ERR_LOGISTIC = 2
 class DeviceSkipGram:
     def __init__(self, vocab: int, dim: int = 300, learning_rate: float = 0.025, negative: int = 5,
                  group=None, seed: int = 0, device: Optional[int] = None,
-                 replica_cache: Optional[bool] = None, sync_every: int = 4):
+                 replica_cache: Optional[bool] = None, sync_every: int = 4, optimizer: str = "sgd"):
+        if optimizer not in ("sgd", "adagrad"):
+            raise ValueError(f"optimizer must be 'sgd' or 'adagrad', got {optimizer!r}")
+        self.optimizer = optimizer
+        ready = dist.is_available() and dist.is_initialized()
+        if optimizer == "adagrad" and (replica_cache or (replica_cache is None and ready
+                                                         and dist.get_world_size(group) > 1)):
+            raise ValueError("optimizer='adagrad' is not supported with the replica cache, the multi-GPU "
+                             "default: pass replica_cache=False to read and update the rows on their owners")
         self.vocab, self.dim, self.lr, self.negative, self.seed = vocab, dim, learning_rate, negative, seed
         b = 0.5 / dim
         self.w_in = ShardedTable(vocab, dim, group=group, device=device, init_range=(-b, b), seed=2 * seed + 1)
@@ -40,6 +50,9 @@ class DeviceSkipGram:
         # (store/replica_cache.py) instead of moving 2 x 1200 B per update over NVLink
         if replica_cache is None:
             replica_cache = self.w_in.world > 1
+        # row-wise AdaGrad state: one fp32 per row of W_in and of W_out, partitioned like the tables
+        self.acc_in = self.w_in.row_accumulators() if optimizer == "adagrad" else None
+        self.acc_out = self.w_out.row_accumulators() if optimizer == "adagrad" else None
         self.rep_in = ReplicaCache(self.w_in, sync_every) if replica_cache else None
         self.rep_out = ReplicaCache(self.w_out, sync_every) if replica_cache else None
         self._ones = None
@@ -58,6 +71,8 @@ class DeviceSkipGram:
                             err_mode=ERR_LOGISTIC, neg_rate=self.negative, num_items=self.vocab,
                             seed=self.seed, step=self.step_no, stats=self.stats, nan_flag=self.nan_flag,
                             kernel="reg",
+                            item_acc=self.acc_out.table_c if self.acc_out else None,
+                            user_acc=self.acc_in.table_c if self.acc_in else None,
                             reserve_total=(self.rep_in.reserve_total() + self.rep_out.reserve_total())
                             if self.rep_in else 0)
         self.step_no += 1
@@ -129,4 +144,6 @@ class DeviceSkipGram:
         gather = getattr(self._neighbours, "_p2p_gather", None)
         if gather is not None:
             gather.close()
+        if self.acc_in is not None:
+            self.acc_in.close(); self.acc_out.close()
         self.w_in.close(); self.w_out.close()

@@ -91,9 +91,11 @@ __device__ __forceinline__ void fps_credit_acquire(int* credits, int n = 1) {
 // chosen by the host from pullLimit (credits pre-distributed to resident lane-groups).
 // ----------------------------------------------------------------------------------------
 
-template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT, int HINT = 0, int EMIT = 0, int LIMIT = 0>
-__global__ void __launch_bounds__(256, MINB)
-    fps_mf_sgd_fused_kernel(const __grid_constant__ MfArgs a) {
+// ADA = 1: row-wise AdaGrad (DESIGN §2.10).  e is taken with learning rate 1, each row's step is
+//   s = |delta|^2 / k,  row += lr * delta / (sqrt(G + s) + eps),  G += s
+// with G the row's accumulator as pulled next to the row.  ADA = 0 is the SGD step, unchanged.
+template <typename IdT, int LPR, int VPL, int R, int FMT, int HINT, int EMIT, int LIMIT, int ADA>
+__device__ __forceinline__ void fps_mf_step_body(const MfArgs& a) {
   unsigned long long pol_user = 0, pol_item = 0;
   if (HINT) {
     pol_user = fps_policy_evict_first();
@@ -122,6 +124,9 @@ __global__ void __launch_bounds__(256, MINB)
     bool ok[R];
     long long uid[R];
     int ncred[R];
+    float* gup[R];
+    float* gvp[R];
+    float gu[R], gv[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       const long long idx = base + (long long)r * n_groups + group;
@@ -173,6 +178,13 @@ __global__ void __launch_bounds__(256, MINB)
                              : a.user_table + fps_user_slot<IdT>(user, a.user_div, a.user_shift) * (size_t)stride;
       vp[r] = fps_row_t<IdT>(a.item_tab, item);
       pp[r] = a.use_push_tab ? fps_row_t<IdT>(a.push_tab, item) : vp[r];
+      if (ADA) {   // the two accumulators, pulled with the rows
+        gup[r] = a.user_sharded ? fps_row_t<IdT>(a.user_acc_tab, user)
+                                : a.user_acc + fps_user_slot<IdT>(user, a.user_div, a.user_shift);
+        gvp[r] = fps_row_t<IdT>(a.item_acc, item);
+        gu[r] = ok[r] ? fps_ld_f32(gup[r]) : 0.f;
+        gv[r] = ok[r] ? fps_ld_f32(gvp[r]) : 0.f;
+      }
 #pragma unroll
       for (int c = 0; c < VPL; ++c) {
         const int q = lane + c * LPR;
@@ -192,21 +204,42 @@ __global__ void __launch_bounds__(256, MINB)
     }
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-      float d = 0.f;
+      float d = 0.f, nu = 0.f, nv = 0.f;
 #pragma unroll
-      for (int c = 0; c < VPL; ++c) d += fps_mf_dot4(u[r][c], v[r][c]);
+      for (int c = 0; c < VPL; ++c) {
+        d += fps_mf_dot4(u[r][c], v[r][c]);
+        if (ADA) {
+          nu += fps_mf_dot4(u[r][c], u[r][c]);
+          nv += fps_mf_dot4(v[r][c], v[r][c]);
+        }
+      }
       d = fps_group_sum<LPR>(d);
       const float resid = rt[r] - d;
-      const float g = fps_mf_grad(a.err_mode, a.lr, rt[r], d, resid);
+      const float g = fps_mf_grad(a.err_mode, ADA ? 1.f : a.lr, rt[r], d, resid);
+      float g_u = g, g_v = g, s_u = 0.f, s_v = 0.f;   // SGD: both rows step by lr * e
+      if (ADA) {   // delta_u = e v, delta_v = e u
+        nu = fps_group_sum<LPR>(nu);
+        nv = fps_group_sum<LPR>(nv);
+        const float ee = g * g / (float)a.item_tab.dim;
+        s_u = ee * nv;
+        s_v = ee * nu;
+        g_u = g * fps_adagrad_scale(a.lr, gu[r], s_u);
+        g_v = g * fps_adagrad_scale(a.lr, gv[r], s_v);
+      }
       if (LIMIT) {
         __syncwarp();                               // every lane holds its part of the answer
         if ((threadIdx.x & 31) == 0 && ncred[r] > 0) atomicAdd(a.credits, ncred[r]);
       }
       if (ok[r]) {
         if (!(fabsf(g) <= 3.0e38f)) bad = true;  // NaN/Inf guard (Vector.scala:78-80)
+        if (ADA && !(fabsf(g_u) <= 3.0e38f && fabsf(g_v) <= 3.0e38f)) bad = true;
         if (lane == 0) {
           sq_acc += resid * resid;
           cnt_acc += 1.f;
+          if (ADA) {
+            fps_red_add1(gup[r], s_u);
+            fps_red_add1(gvp[r], s_v);
+          }
         }
         long long out_slot = -1;
         if (EMIT) {   // E5: this update's view of the new user vector goes to the output staging area
@@ -221,8 +254,8 @@ __global__ void __launch_bounds__(256, MINB)
         for (int c = 0; c < VPL; ++c) {
           const int q = lane + c * LPR;
           if (q < nvec) {
-            float4 du = make_float4(g * v[r][c].x, g * v[r][c].y, g * v[r][c].z, g * v[r][c].w);
-            float4 dv = make_float4(g * u[r][c].x, g * u[r][c].y, g * u[r][c].z, g * u[r][c].w);
+            float4 du = make_float4(g_u * v[r][c].x, g_u * v[r][c].y, g_u * v[r][c].z, g_u * v[r][c].w);
+            float4 dv = make_float4(g_v * u[r][c].x, g_v * u[r][c].y, g_v * u[r][c].z, g_v * u[r][c].w);
             if (EMIT && out_slot >= 0)
               *reinterpret_cast<float4*>(a.out_vecs + out_slot * (long long)stride + 4 * q) =
                   make_float4(u[r][c].x + du.x, u[r][c].y + du.y, u[r][c].z + du.z, u[r][c].w + du.w);
@@ -251,18 +284,35 @@ __global__ void __launch_bounds__(256, MINB)
   if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
 }
 
+template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT, int HINT = 0, int EMIT = 0, int LIMIT = 0>
+__global__ void __launch_bounds__(256, MINB)
+    fps_mf_sgd_fused_kernel(const __grid_constant__ MfArgs a) {
+  fps_mf_step_body<IdT, LPR, VPL, R, FMT, HINT, EMIT, LIMIT, 0>(a);
+}
+
+// Row-wise AdaGrad family: the default register-staged geometries only (no L2 hints, output stream or
+// credit counter; a pull limit is the static capped grid).
+template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT>
+__global__ void __launch_bounds__(256, MINB)
+    fps_mf_adagrad_fused_kernel(const __grid_constant__ MfArgs a) {
+  fps_mf_step_body<IdT, LPR, VPL, R, FMT, 0, 0, 0, 1>(a);
+}
+
 static int g_mf_reserve = 0;        // CTA slots per SM left free for a concurrently running kernel
 static int g_mf_reserve_total = 0;  // CTA slots left free on the whole GPU (the replica exchange CTAs)
 extern "C" void fps_set_mf_reserve(int v) { g_mf_reserve = v < 0 ? 0 : v; }
 extern "C" void fps_set_mf_reserve_total(int v) { g_mf_reserve_total = v < 0 ? 0 : v; }
 
-template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT, int HINT = 0, int EMIT = 0, int LIMIT = 0>
+template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT, int HINT = 0, int EMIT = 0, int LIMIT = 0,
+          int ADA = 0>
 static int launch_mf(const MfArgs& a, int max_inflight_rows, int num_sms, cudaStream_t stream) {
   const int threads = 256;
   const int groups_per_block = threads / LPR;
+  void (*kern)(const MfArgs);
+  if constexpr (ADA) kern = fps_mf_adagrad_fused_kernel<IdT, LPR, VPL, R, MINB, FMT>;
+  else kern = fps_mf_sgd_fused_kernel<IdT, LPR, VPL, R, MINB, FMT, HINT, EMIT, LIMIT>;
   int occ = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(
-      &occ, fps_mf_sgd_fused_kernel<IdT, LPR, VPL, R, MINB, FMT, HINT, EMIT, LIMIT>, threads, 0);
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, 0);
   occ -= g_mf_reserve;  // leave slots for the background replica exchange (see fps_cache_sync)
   if (occ < 1) occ = 1;
   long long blocks = (long long)num_sms * occ - g_mf_reserve_total;
@@ -277,7 +327,7 @@ static int launch_mf(const MfArgs& a, int max_inflight_rows, int num_sms, cudaSt
   long long need = (n_eff + (long long)groups_per_block * R - 1) / ((long long)groups_per_block * R);
   if (need < 1) need = 1;
   if (blocks > need) blocks = need;
-  fps_mf_sgd_fused_kernel<IdT, LPR, VPL, R, MINB, FMT, HINT, EMIT, LIMIT><<<(int)blocks, threads, 0, stream>>>(a);
+  kern<<<(int)blocks, threads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
 
@@ -290,6 +340,20 @@ template <typename IdT, int FMT>
 static int dispatch_mf(const MfArgs& a, int max_inflight, int num_sms, cudaStream_t s) {
   const int nvec = a.item_tab.stride >> 2;
   const int v = g_mf_reg_variant;
+  if (a.item_acc.base[0] != nullptr) {   // row-wise AdaGrad: the default geometries, 0 spills (ptxas -v)
+    if (a.credits != nullptr || a.out_every > 0 || a.use_push_tab) return -1009;
+    if (nvec <= 1) return launch_mf<IdT, 1, 1, 2, 4, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    if (nvec <= 2) return launch_mf<IdT, 2, 1, 2, 4, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    if (nvec <= 4) return launch_mf<IdT, 4, 1, 2, 4, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    if (nvec <= 8) return launch_mf<IdT, 8, 1, 1, 6, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    if (nvec <= 16) return launch_mf<IdT, 16, 1, 1, 6, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    if (nvec <= 32) return launch_mf<IdT, 32, 1, 1, 6, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    if (nvec <= 64) return launch_mf<IdT, 32, 2, 1, 4, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    if (nvec <= 96) return launch_mf<IdT, 32, 3, 1, 4, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    if (nvec <= 128) return launch_mf<IdT, 32, 4, 1, 2, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    if (nvec <= 256) return launch_mf<IdT, 32, 8, 1, 2, FMT, 0, 0, 0, 1>(a, max_inflight, num_sms, s);
+    return -1000;
+  }
   if (a.credits != nullptr) {   // device credit-counter pull limiter: the counter bounds the pulls in flight;
     const int cap = 2 * max_inflight;  // the grid is trimmed to ~2x the credits (fewer contenders on the counter)
     if (nvec <= 4) return launch_mf<IdT, 4, 1, 1, 4, FMT, 0, 0, 1>(a, cap, num_sms, s);

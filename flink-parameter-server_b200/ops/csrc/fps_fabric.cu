@@ -67,6 +67,7 @@ extern "C" int fps_device_info(int dev, int* sm_count, int* cc_major, int* cc_mi
 extern "C" const char* fps_error_string(int code) {
   if (code == -1000) return "dim too large for fused kernel";
   if (code == -1001) return "unsupported id width";
+  if (code == -1009) return "row-wise AdaGrad does not support this kernel variant";
   if (code < 0) return "fps: invalid argument";
   return cudaGetErrorString((cudaError_t)code);
 }

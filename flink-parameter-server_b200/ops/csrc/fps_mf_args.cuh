@@ -42,7 +42,26 @@ struct MfArgs {
   int pad3_;
   int* credits;              // device-side pull limiter (WL:196-250): credits[0] = pulls that may still be
                              //   issued, credits[1] = stall counter; nullptr = unlimited
+  // Row-wise AdaGrad (one fp32 accumulator per row, partitioned like its table; stride 1).
+  // item_acc.base[0] == nullptr means plain SGD.
+  ShardTable item_acc;       // item accumulators, addressed like item_tab (peer shards over NVLink)
+  ShardTable user_acc_tab;   // user accumulators when user_sharded != 0 (skip-gram W_in)
+  float* user_acc;           // worker-local [n_local_users] user accumulators otherwise
 };
+
+// Row-wise AdaGrad accumulator access: a scalar load of G as pulled, and the one-sided G += s.
+__device__ __forceinline__ float fps_ld_f32(const float* p) {
+  float v;
+  asm volatile("ld.global.f32 %0, [%1];" : "=f"(v) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ void fps_red_add1(float* p, float v) {
+  asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+}
+// lr / (sqrt(G + s) + eps): the step of a row whose accumulator read G and whose squared delta mean is s
+__device__ __forceinline__ float fps_adagrad_scale(float lr, float G, float s) {
+  return lr / (sqrtf(G + s) + 1e-8f);
+}
 
 // The pointwise update rule, shared by every fp32 kernel that applies it (fps_core.cu per-launch kernel,
 // fps_mf_window.cu windowed drain): one lane's part of u.v, and the step g = lr * e from the group's dot.

@@ -79,6 +79,9 @@ class MfArgsC(C.Structure):
         ("out_every", C.c_int),
         ("pad3_", C.c_int),
         ("credits", C.c_void_p),
+        ("item_acc", ShardTableC),
+        ("user_acc_tab", ShardTableC),
+        ("user_acc", C.c_void_p),
     ]
 
 
@@ -243,8 +246,14 @@ def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
                  kernel: Optional[str] = None, push_tab: Optional[ShardTableC] = None,
                  l2_hints: bool = False, reserve_ctas: int = 0, reserve_total: int = 0,
                  progress: Optional[torch.Tensor] = None, output=None,
-                 credits: Optional[torch.Tensor] = None) -> None:
+                 credits: Optional[torch.Tensor] = None, item_acc: Optional[ShardTableC] = None,
+                 user_acc=None) -> None:
     """Fused pull + SGD + push (K1+K3+K2).
+
+    ``item_acc`` / ``user_acc``: row-wise AdaGrad instead of SGD (DESIGN §2.10).  ``item_acc`` is a stride-1
+    :class:`ShardTableC` of one fp32 accumulator per item row, partitioned like ``item_tab``; ``user_acc`` is
+    a float32 ``[n_local]`` tensor, or a stride-1 :class:`ShardTableC` when ``user_table`` is one.  AdaGrad
+    runs on the register-staged kernel only, without ``push_tab``, ``output`` or ``credits``.
 
     ``kernel="reg"`` (default): register-staged loads at full occupancy (csrc/fps_core.cu);
     ``kernel="tma"``: warp-specialised TMA/mbarrier pipeline (csrc/fps_mf_tma.cu) -- slower for
@@ -295,6 +304,26 @@ def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
         o_ids, o_vecs, o_staged, o_cap, o_every = output
         a.out_ids = o_ids.data_ptr(); a.out_vecs = o_vecs.data_ptr(); a.out_staged = o_staged.data_ptr()
         a.out_cap = int(o_cap); a.out_every = int(o_every)
+    if item_acc is not None:
+        if push_tab is not None or output is not None or credits is not None:
+            raise ValueError("row-wise AdaGrad does not support push_tab, output or credits")
+        if int(item_acc.stride) != 1:
+            raise ValueError("item_acc must be a stride-1 accumulator table")
+        a.item_acc = item_acc
+        if user_sharded:
+            if not isinstance(user_acc, ShardTableC) or int(user_acc.stride) != 1:
+                raise ValueError("a sharded user table needs a stride-1 ShardTableC user_acc")
+            a.user_acc_tab = user_acc
+        else:
+            if not torch.is_tensor(user_acc):
+                raise ValueError("a worker-local user table needs a float32 user_acc tensor")
+            _req(user_acc, "user_acc", torch.float32)
+            if user_acc.numel() < user_table.shape[0]:
+                raise ValueError("user_acc must hold one accumulator per user row")
+            a.user_acc = user_acc.data_ptr()
+        variant = "reg"
+    elif user_acc is not None:
+        raise ValueError("user_acc needs item_acc")
     lib().fps_set_mf_reserve(int(reserve_ctas))
     lib().fps_set_mf_reserve_total(int(reserve_total))
     rv = os.environ.get("FPS_MF_REG_VARIANT")
@@ -381,6 +410,7 @@ class BprArgsC(C.Structure):
         ("cand_table", C.c_void_p), ("cand_div", C.c_int), ("cand_shift", C.c_int), ("cand_tab", ShardTableC),
         ("use_push_tab", C.c_int), ("stride", C.c_int), ("push_tab", ShardTableC),
         ("stats", C.c_void_p), ("nan_flag", C.c_void_p), ("reserve_total", C.c_int), ("pad_", C.c_int),
+        ("anchor_acc_tab", ShardTableC), ("cand_acc", ShardTableC), ("anchor_acc", C.c_void_p),
     ]
 
 
@@ -390,7 +420,7 @@ def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Op
                  seed: int = 0, step: int = 0, anchor_div: int = 1, cand_div: int = 1,
                  stats: Optional[torch.Tensor] = None, nan_flag: Optional[torch.Tensor] = None,
                  max_inflight_rows: int = 0, push_tab: Optional[ShardTableC] = None,
-                 reserve_total: int = 0) -> None:
+                 reserve_total: int = 0, anchor_acc=None, cand_acc: Optional[ShardTableC] = None) -> None:
     """Fused pairwise (BPR) pull + SGD + push, one ``(anchor, positive, negative)`` triple per update
     (csrc/fps_mf_bpr.cu).  ``users`` are the anchor ids, ``items`` the positive candidates; records with
     ``rating <= 0`` are skipped.  ``items=None``: ``users`` holds packed64 records (:func:`pack_ratings`).
@@ -404,7 +434,12 @@ def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Op
     ``[0, num_items)`` and never the positive.  ``stats`` (float32 ``[3]``) accumulates the softplus loss
     sum, the number of triples and the number with ``x > 0``.  ``max_inflight_rows`` caps the grid so that
     at most that many rows are being pulled at once (3 per lane-group).  ``reserve_total``: CTA slots
-    the grid leaves free for a kernel running next to it (the replica exchange)."""
+    the grid leaves free for a kernel running next to it (the replica exchange).
+
+    ``cand_acc`` / ``anchor_acc``: row-wise AdaGrad instead of SGD (DESIGN §2.10).  ``cand_acc`` is a stride-1
+    :class:`ShardTableC` of candidate accumulators (``cand_table`` must then be a ShardTableC, without
+    ``push_tab``); ``anchor_acc`` a float32 ``[rows]`` tensor, or a stride-1 ShardTableC when ``anchor_table``
+    is one."""
     _req(users, "users")
     packed = items is None
     if packed:
@@ -463,6 +498,25 @@ def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Op
     a.n_pos = n_pos; a.num_items = int(max(num_items, 1))
     a.seed = seed & (2**64 - 1); a.step = int(step)
     a.lr = float(lr); a.reg = float(reg); a.reserve_total = int(reserve_total)
+    if cand_acc is not None:
+        if not a.cand_sharded or push_tab is not None:
+            raise ValueError("row-wise AdaGrad needs a ShardTableC cand_table and no push_tab")
+        if int(cand_acc.stride) != 1:
+            raise ValueError("cand_acc must be a stride-1 accumulator table")
+        a.cand_acc = cand_acc
+        if a.anchor_sharded:
+            if not isinstance(anchor_acc, ShardTableC) or int(anchor_acc.stride) != 1:
+                raise ValueError("a sharded anchor table needs a stride-1 ShardTableC anchor_acc")
+            a.anchor_acc_tab = anchor_acc
+        else:
+            if not torch.is_tensor(anchor_acc):
+                raise ValueError("a worker-local anchor table needs a float32 anchor_acc tensor")
+            _req(anchor_acc, "anchor_acc", torch.float32)
+            if anchor_acc.numel() < anchor_table.shape[0]:
+                raise ValueError("anchor_acc must hold one accumulator per anchor row")
+            a.anchor_acc = anchor_acc.data_ptr()
+    elif anchor_acc is not None:
+        raise ValueError("anchor_acc needs cand_acc")
     _check(lib().fps_mf_bpr_fused(C.byref(a), 4 if packed else _id_bytes(users), int(max_inflight_rows),
                                   sm_count(users.device.index), _stream()), "mf_bpr_fused")
     _bump()

@@ -215,3 +215,43 @@ class ShardedTable:
 
     def close(self) -> None:
         self.heap.close()
+
+    def row_accumulators(self) -> "RowAccumulators":
+        """One zeroed fp32 per row of this table, partitioned exactly like it (row-wise AdaGrad state)."""
+        return RowAccumulators(self)
+
+
+class RowAccumulators:
+    """Per-row optimizer state of a :class:`ShardedTable`: a ``[rows_per_shard]`` fp32 block per shard in its
+    own symmetric heap, so peers read and reduce it the way they reach the rows.  ``table_c`` addresses it
+    with the table's partitioning and stride 1; ``local`` is this rank's block."""
+
+    def __init__(self, table: ShardedTable):
+        self.table = table
+        self.heap = SymmetricHeap(table.rows_per_shard * 4, group=table.group, device=table.device,
+                                  mode=table.heap.mode)
+        self.local = self.heap.local_tensor((table.rows_per_shard,), torch.float32)
+        src = table.table_c
+        tc = native.ShardTableC()
+        for r in range(table.n_shards):
+            tc.base[r] = self.heap.peer_ptrs[r]
+        tc.rows_per_shard, tc.div, tc.num_shards = src.rows_per_shard, src.div, src.num_shards
+        tc.dim, tc.stride, tc.mode, tc.shard_shift, tc.lut = 1, 1, src.mode, src.shard_shift, src.lut
+        self.table_c = tc
+        self.heap.barrier()
+
+    def dump_local(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        """(ids, accumulators) of the local shard's valid rows."""
+        torch.cuda.synchronize(self.table.device)
+        ids = self.table.local_ids()
+        sel = (ids < self.table.num_ids).nonzero(as_tuple=True)[0]
+        return ids[sel], self.local[sel].clone()
+
+    def load(self, ids: torch.Tensor, values: torch.Tensor) -> None:
+        """Overwrite the local shard's accumulators of ``ids`` (ids this rank owns)."""
+        t = self.table
+        slots = ids // t.n_shards if t.mode == native.PART_HASH else ids - t.rank * t.div
+        self.local[slots] = values.to(self.local.device, torch.float32)
+
+    def close(self) -> None:
+        self.heap.close()
