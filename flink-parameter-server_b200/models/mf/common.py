@@ -217,6 +217,53 @@ def require_pointwise(backend: str, kw: dict) -> None:
     if backend != "device" and kw.get("optimizer", "sgd") != "sgd":
         raise ValueError(f"optimizer={kw.get('optimizer')!r} needs backend='device' "
                          f"(backend={backend!r} trains with SGD only)")
+    ns = kw.get("negativeSampling")
+    if ns is not None and ns not in ("uniform", "seen"):
+        raise ValueError(f"negativeSampling must be 'uniform' or 'seen', got {ns!r}")
+    if backend != "device" and ns == "uniform":
+        raise ValueError(f"negativeSampling='uniform' needs backend='device' (backend={backend!r} samples "
+                         f"negatives from the items each worker has seen: negativeSampling='seen')")
+
+
+class SeenRegistryOracle:
+    """numpy reference of the device's seen-items registry (``negative_sampling="seen"``, DESIGN §2.11), the rule
+    of PSOnlineMatrixFactorizationWorker.scala:61-88 and ops/csrc/fps_host.cpp:216-249 applied per micro-batch.
+
+    :meth:`batch` takes one micro-batch ``(users, items)`` in stream order and returns, per record, ``|D_p|`` (the
+    items seen before it: the registry before the batch plus the batch's items first seen at earlier
+    positions), ``|ring_p|`` (the user's ratings so far, this one included, capped at ``user_memory``) and the
+    negative count ``max(0, min(|D_p| - |ring_p|, neg_rate))``; then registers the batch's new items.  ``order``
+    holds the registered items in first-occurrence order.  ``user_div``: users are counted per
+    ``user // user_div`` slot, like the device ring."""
+
+    def __init__(self, num_items: int, num_users: int, neg_rate: int, user_memory: int, user_div: int = 1):
+        self.neg_rate, self.memory, self.user_div = int(neg_rate), int(user_memory), int(user_div)
+        self.known = np.zeros(int(num_items), dtype=bool)
+        self.order = np.zeros(0, dtype=np.int64)
+        self.user_count = np.zeros(-(-int(num_users) // self.user_div), dtype=np.int64)
+
+    def batch(self, users, items):
+        users = np.asarray(users, dtype=np.int64) // self.user_div
+        items = np.asarray(items, dtype=np.int64)
+        n = items.size
+        _, first = np.unique(items, return_index=True)
+        flag = np.zeros(n, dtype=bool)
+        flag[first] = True
+        flag &= ~self.known[items]
+        dom = self.order.size + np.cumsum(flag) - flag
+        # ratings of the same user earlier in the batch: rank inside the stable sort by user
+        by_user = np.argsort(users, kind="stable")
+        su = users[by_user]
+        start = np.r_[True, su[1:] != su[:-1]] if n else np.zeros(0, dtype=bool)
+        rank = np.arange(n) - np.maximum.accumulate(np.where(start, np.arange(n), 0))
+        within = np.empty(n, dtype=np.int64)
+        within[by_user] = rank
+        ring = np.minimum(self.user_count[users] + within + 1, self.memory)
+        k_neg = np.clip(dom - ring, 0, self.neg_rate)
+        np.add.at(self.user_count, users, 1)
+        self.order = np.concatenate([self.order, items[flag]])
+        self.known[items] = True
+        return dom, ring, k_neg
 
 
 # ---- top-K ------------------------------------------------------------------------------

@@ -60,6 +60,24 @@ def check_optimizer(optimizer: str, *, item_cache: bool, output_ring=None, kerne
         raise ValueError("optimizer='adagrad' runs on the register-staged kernel: pass kernel=None or 'reg'")
 
 
+NEGATIVE_SAMPLING = ("uniform", "seen")
+
+
+def check_negative_sampling(negative_sampling: str, negative_sample_rate: int, negatives=None) -> None:
+    """Raise ``ValueError`` for a negative-sampling setting :class:`DeviceOnlineMF` cannot run.  ``"seen"`` draws
+    the negatives itself from the items the worker has seen, so it needs a positive ``negative_sample_rate`` and
+    takes no ``step(negatives=...)``."""
+    if negative_sampling not in NEGATIVE_SAMPLING:
+        raise ValueError(f"negative_sampling must be 'uniform' or 'seen', got {negative_sampling!r}")
+    if negative_sampling != "seen":
+        return
+    if int(negative_sample_rate) < 1:
+        raise ValueError("negative_sampling='seen' needs negative_sample_rate >= 1 (or negative_sampling='uniform')")
+    if negatives is not None:
+        raise ValueError("negative_sampling='seen' draws the negatives itself: call step() without negatives=, or "
+                         "use negative_sampling='uniform' to pass explicit negatives")
+
+
 def step_window_size(step_window: Optional[int], *, world: int, item_cache: bool, loss: str, table_rows: int,
                      stride: int, env: Optional[str] = None, optimizer: str = "sgd") -> int:
     """Micro-batches per step window of :class:`DeviceOnlineMF` (0 = off).
@@ -108,7 +126,8 @@ class DeviceOnlineMF:
                  block_bytes: int = 16 << 20, flush_count: Optional[int] = None,
                  flush_require: str = "any", replica_own_inplace: Optional[bool] = None,
                  output_ring=None, loss: str = "pointwise", regularization: float = 0.0,
-                 step_window: Optional[int] = None, optimizer: str = "sgd"):
+                 step_window: Optional[int] = None, optimizer: str = "sgd",
+                 negative_sampling: str = "uniform"):
         """``loss="bpr"``: pairwise (Bayesian Personalised Ranking) updates, each positive rating paired
         with ``negative_sample_rate`` negatives (sampled) or with the ``negatives=`` of :meth:`step`;
         ``regularization`` is its L2 weight.  The pointwise loss has no regulariser.
@@ -119,9 +138,18 @@ class DeviceOnlineMF:
         ``optimizer="adagrad"``: row-wise AdaGrad (DESIGN §2.10) instead of SGD with one global rate.  Each row
         keeps one fp32 accumulator ``G`` of its mean squared delta and steps by ``learning_rate / (sqrt(G) +
         1e-8)``; users' accumulators stay on their worker, items' on the item's shard.  It runs per launch (no
-        step window) in the direct mode only: ``item_cache=False`` when there is more than one GPU."""
+        step window) in the direct mode only: ``item_cache=False`` when there is more than one GPU.
+
+        ``negative_sampling``: where negatives come from.  ``"uniform"`` draws them uniformly over ``[0,
+        num_items)``.  ``"seen"`` draws them, as the reference and the host tiers do, from the items this worker
+        has seen so far (DESIGN §2.11): a device registry keeps them in first-occurrence order (see
+        :meth:`seen_items`), rating ``p`` of a micro-batch samples from the items seen before it, rejecting the
+        user's last ``user_memory`` items and the positive, and gets ``min(negative_sample_rate, |domain| -
+        |user's recent items|)`` negatives.  It needs ``negative_sample_rate >= 1``."""
         self._pending = []           # staged micro-batches of the step window: (records, format)
         self.step_window = 0
+        check_negative_sampling(negative_sampling, negative_sample_rate)
+        self.negative_sampling = negative_sampling
         if loss not in ("pointwise", "bpr"):
             raise ValueError(f"loss must be 'pointwise' or 'bpr', got {loss!r}")
         self.loss, self.reg = loss, float(regularization)
@@ -188,6 +216,9 @@ class DeviceOnlineMF:
                 self.seen = torch.full((n_local, self.user_memory), -1, dtype=torch.int32,
                                        device=self.cuda_device)
                 self.seen_pos = torch.zeros(n_local, dtype=torch.int32, device=self.cuda_device)
+            # negative_sampling="seen": the items this worker has seen, in first-occurrence order
+            self._registry = (native.seen_registry(self.num_items, self.cuda_device)
+                              if negative_sampling == "seen" else None)
         # ---- item-cache mode (sender-side combining) --------------------------------------------
         # The worker trains a local owner-major replica of the item table (pulls and pushes stay in local
         # HBM); its segments are the per-destination send buffers of the reference's batching senders.
@@ -210,7 +241,7 @@ class DeviceOnlineMF:
         row_bytes = self._items.stride * 4
         if item_blocking is None:
             item_blocking = ((self.world == 1 or self.item_cache) and self.num_items * row_bytes > (48 << 20)
-                             and (self.neg == 0 or self.user_memory > 0)
+                             and (self.neg == 0 or self.user_memory > 0 or negative_sampling == "seen")
                              and os.environ.get("FPS_ITEM_BLOCKING", "1") != "0")
         self.item_blocking = bool(item_blocking)
         block_bytes = int(os.environ.get("FPS_BLOCK_BYTES", block_bytes))
@@ -350,18 +381,17 @@ class DeviceOnlineMF:
                 self._drain()
             return
         self._drain()
+        check_negative_sampling(self.negative_sampling, self.neg, negatives)
         if self.loss == "bpr":
             self._step_bpr(users, items, ratings, negatives)
             return
         if negatives is not None:
             raise ValueError("negatives= needs loss='bpr'")
         neg = self.neg
-        if self.user_memory > 0:
-            # negatives drawn by the sampler kernel against the per-user seen ring; the fused kernel
+        if self.user_memory > 0 or self._registry is not None:
+            # negatives drawn by a sampler kernel (the per-user seen ring, the seen-items registry); the fused kernel
             # then consumes the expanded batch as plain records
-            users, items, ratings = native.neg_sample(users, items, ratings, self.neg, self.num_items,
-                                                      self.seen, self.seen_pos, self.world,
-                                                      seed=self.seed, step=self.step_no)
+            users, items, ratings = self._sample_negatives(users, items, ratings)
             neg = 0
         n_records = users.numel()
         fed = False
@@ -411,12 +441,11 @@ class DeviceOnlineMF:
             n = int(negatives.shape[1]) if negatives.dim() == 2 else 0
         elif self.neg < 1:
             raise ValueError("loss='bpr' needs negative_sample_rate >= 1 or explicit negatives=")
-        elif self.user_memory > 0:
+        elif self.user_memory > 0 or self._registry is not None:
             # negatives that avoid the user's recent items: the sampler's expanded [n, 1 + m] records,
             # with the negatives it could not find voided
             per = 1 + self.neg
-            ou, oi, orat = native.neg_sample(users, items, ratings, self.neg, self.num_items, self.seen,
-                                             self.seen_pos, self.world, seed=self.seed, step=self.step_no)
+            ou, oi, orat = self._sample_negatives(users, items, ratings)
             ou, oi = ou.view(-1, per), oi.view(-1, per)
             negatives = torch.where(ou[:, 1:] >= 0, oi[:, 1:], torch.full_like(oi[:, 1:], -1)).contiguous()
             users, items, ratings = ou[:, 0].contiguous(), oi[:, 0].contiguous(), orat.view(-1, per)[:, 0].contiguous()
@@ -439,6 +468,24 @@ class DeviceOnlineMF:
                             cand_acc=self._item_acc.table_c if self._item_acc is not None else None)
         self.step_no += 1
         METRICS.inc("mf_ratings", n_pos)
+
+    def _sample_negatives(self, users, items, ratings):
+        """Expanded ``(users, items, ratings)`` records: each rating, then its ``negative_sample_rate`` negatives."""
+        memory = self.user_memory > 0
+        if self._registry is not None:
+            return native.neg_sample_seen(users, items, ratings, self.neg, self._registry,
+                                          self.seen if memory else None, self.seen_pos if memory else None,
+                                          self.world, seed=self.seed, step=self.step_no)
+        return native.neg_sample(users, items, ratings, self.neg, self.num_items, self.seen, self.seen_pos,
+                                 self.world, seed=self.seed, step=self.step_no)
+
+    def seen_items(self) -> torch.Tensor:
+        """The item ids this worker has seen, in first-occurrence order (int64, on the device); the domain of
+        ``negative_sampling="seen"``.  Raises ``ValueError`` with ``negative_sampling="uniform"``."""
+        if self._registry is None:
+            raise ValueError("seen_items() needs negative_sampling='seen'")
+        order, count, _ = self._registry
+        return order[:int(count.item())].to(torch.int64)
 
     def make_graph_step(self, batch_size: int, packed: bool = True):
         """CUDA-graph a fixed-size micro-batch step for launch-bound streaming (small batches).

@@ -74,7 +74,7 @@ def ps_online_mf_device(src, numFactors=10, rangeMin=-0.01, rangeMax=0.01, learn
                         userMemory: int = 128, updateOutput: Optional[int] = None,
                         outputFlushCount: int = 1, outputFlushMs: Optional[float] = None,
                         loss: str = "pointwise", regularization: float = 0.0,
-                        optimizer: str = "sgd") -> ResultStream:
+                        optimizer: str = "sgd", negativeSampling: Optional[str] = None) -> ResultStream:
     """``updateOutput=n``: also emit ``Left((userId, userVector))`` for one update in ``n`` (``1`` = every
     update, the reference's worker output PSOnlineMatrixFactorizationWorker.scala:52) through the device
     output ring (count / timer flushed on the device); the final dump then holds only the item shard.
@@ -82,7 +82,10 @@ def ps_online_mf_device(src, numFactors=10, rangeMin=-0.01, rangeMax=0.01, learn
     negatives, L2 weight ``regularization`` (see :class:`DeviceOnlineMF`); it has no per-update output,
     so ``updateOutput`` with ``loss="bpr"`` raises ``ValueError``.
     ``optimizer="adagrad"``: row-wise AdaGrad (see :class:`DeviceOnlineMF`); a multi-rank job then reads and
-    updates the item rows on their owners (no item cache)."""
+    updates the item rows on their owners (no item cache).
+    ``negativeSampling="seen"``: negatives from the items each rank has seen so far, the rule of the reference and
+    the host tiers (see :class:`DeviceOnlineMF`); the registry of seen items carries over from epoch to epoch.
+    ``None`` or ``"uniform"``: uniform over the whole item range."""
     if updateOutput and loss != "pointwise":
         raise ValueError("updateOutput (the per-update output ring) is not supported with loss='bpr'")
     recs = None
@@ -101,7 +104,8 @@ def ps_online_mf_device(src, numFactors=10, rangeMin=-0.01, rangeMax=0.01, learn
                            track_touched=True,
                            user_memory=min(int(userMemory), 256) if negativeSampleRate > 0 else 0,
                            loss=loss, regularization=regularization, optimizer=optimizer,
-                           item_cache=False if optimizer == "adagrad" else None)
+                           item_cache=False if optimizer == "adagrad" else None,
+                           negative_sampling=negativeSampling or "uniform")
     ring, updates = None, []
     if updateOutput:
         from ...runtime.output_ring import OutputRing

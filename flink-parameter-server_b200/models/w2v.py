@@ -9,12 +9,15 @@ from their owners, and pushes ``g*v`` to ``W_in[center]`` and ``g*u`` to ``W_out
 ``negative`` extra pairs per positive are sampled on the device (uniform over the vocabulary) with
 label 0.  Not part of the reference's algorithm suite; it exercises the same API on a 1.2 KB row.
 ``optimizer="adagrad"`` replaces the global rate by row-wise AdaGrad (DESIGN §2.10), with one fp32
-accumulator per row of each table on that row's shard.
+accumulator per row of each table on that row's shard.  ``noise_counts`` draws the negatives from the unigram
+noise ``counts ** noise_power`` (Mikolov et al. 2013) instead (DESIGN §2.11).
 """
 from __future__ import annotations
 
+import math
 from typing import Optional
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -26,10 +29,33 @@ from ..store.sharded_table import ShardedTable
 ERR_LOGISTIC = 2
 
 
+def check_noise(noise_counts, vocab: int, noise_power: float) -> np.ndarray:
+    """Validate the unigram counts of :class:`DeviceSkipGram` and return them as float64: one finite,
+    non-negative count per word, not all zero, and a finite ``noise_power >= 0``.  Raises ``ValueError``."""
+    if not (math.isfinite(float(noise_power)) and float(noise_power) >= 0):
+        raise ValueError(f"noise_power must be a finite number >= 0, got {noise_power!r}")
+    c = (noise_counts.detach().cpu().numpy() if torch.is_tensor(noise_counts)
+         else np.asarray(noise_counts)).astype(np.float64).reshape(-1)
+    if c.size != int(vocab):
+        raise ValueError(f"noise_counts must hold one count per word of the vocabulary ({vocab}), got {c.size}")
+    if not np.isfinite(c).all():
+        raise ValueError("noise_counts must be finite")
+    if (c < 0).any():
+        raise ValueError("noise_counts must be >= 0")
+    if not (c > 0).any():
+        raise ValueError("noise_counts must have a positive count for at least one word")
+    return c
+
+
 class DeviceSkipGram:
     def __init__(self, vocab: int, dim: int = 300, learning_rate: float = 0.025, negative: int = 5,
                  group=None, seed: int = 0, device: Optional[int] = None,
-                 replica_cache: Optional[bool] = None, sync_every: int = 4, optimizer: str = "sgd"):
+                 replica_cache: Optional[bool] = None, sync_every: int = 4, optimizer: str = "sgd",
+                 noise_counts=None, noise_power: float = 0.75):
+        """``noise_counts``: ``[vocab]`` word counts.  The negatives are then drawn from ``counts ** noise_power``
+        (0.75 is word2vec's choice; words of count 0 are never drawn) by a sampler kernel over an fp64 inverse
+        CDF, instead of uniformly over the vocabulary inside the training kernel.  ``None`` = uniform."""
+        noise = check_noise(noise_counts, vocab, noise_power) if noise_counts is not None else None
         if optimizer not in ("sgd", "adagrad"):
             raise ValueError(f"optimizer must be 'sgd' or 'adagrad', got {optimizer!r}")
         self.optimizer = optimizer
@@ -58,6 +84,13 @@ class DeviceSkipGram:
         self._ones = None
         self._neighbours = None   # most_similar's scorer over the normalised W_in shard
         self._snapshot_step = -1  # step_no the normalised snapshot was taken at
+        # unigram noise: the fp64 inverse CDF of counts ** noise_power and the last word it can return
+        self.noise_power = float(noise_power)
+        self._noise_cdf, self._noise_last = None, 0
+        if noise is not None:
+            with torch.cuda.device(self.dev):
+                self._noise_cdf = native.noise_cdf(torch.from_numpy(noise).to(self.dev), self.noise_power)
+            self._noise_last = int(np.flatnonzero(noise > 0)[-1])
 
     def step(self, centers: torch.Tensor, contexts: torch.Tensor) -> None:
         if self._ones is None or self._ones.numel() != centers.numel():
@@ -67,8 +100,14 @@ class DeviceSkipGram:
         if self.rep_in:   # policy + exchange kernels first (side streams), then the training kernel
             n = centers.numel() * (1 + self.negative)
             self.rep_in.after_step(n); self.rep_out.after_step(n)
-        native.mf_sgd_fused(centers, contexts, self._ones, tin, 1, tout, self.lr,
-                            err_mode=ERR_LOGISTIC, neg_rate=self.negative, num_items=self.vocab,
+        labels, neg = self._ones, self.negative
+        if self._noise_cdf is not None and neg > 0:
+            # expanded (center, word, label) records: each pair, then its negatives drawn from the noise
+            centers, contexts, labels = native.neg_sample_noise(centers, contexts, self._ones, neg, self._noise_cdf,
+                                                                self._noise_last, seed=self.seed, step=self.step_no)
+            neg = 0
+        native.mf_sgd_fused(centers, contexts, labels, tin, 1, tout, self.lr,
+                            err_mode=ERR_LOGISTIC, neg_rate=neg, num_items=self.vocab,
                             seed=self.seed, step=self.step_no, stats=self.stats, nan_flag=self.nan_flag,
                             kernel="reg",
                             item_acc=self.acc_out.table_c if self.acc_out else None,

@@ -607,6 +607,127 @@ def neg_sample(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Opti
     return ou, oi, orat
 
 
+class NegDomainArgsC(C.Structure):
+    """Mirror of ``struct NegDomainArgs`` (csrc/fps_negatives.cu)."""
+
+    _fields_ = [
+        ("users", C.c_void_p), ("items", C.c_void_p), ("ratings", C.c_void_p),
+        ("n_pos", C.c_longlong), ("neg_rate", C.c_int), ("format", C.c_int),
+        ("seed", C.c_ulonglong), ("step", C.c_ulonglong), ("max_tries", C.c_int),
+        ("memory", C.c_int), ("seen", C.c_void_p), ("seen_pos", C.c_void_p), ("user_div", C.c_int),
+        ("cta_cap", C.c_int), ("num_items", C.c_longlong), ("order", C.c_void_p), ("count", C.c_void_p),
+        ("first_pos", C.c_void_p), ("scratch", C.c_void_p), ("cta_new", C.c_void_p),
+        ("cdf", C.c_void_p), ("vocab", C.c_longlong), ("last_nonzero", C.c_longlong),
+        ("out_users", C.c_void_p), ("out_items", C.c_void_p), ("out_ratings", C.c_void_p),
+    ]
+
+
+def _neg_domain_args(users, items, ratings, neg_rate: int, seed: int, step: int, max_tries: int):
+    _req(users, "users")
+    packed = items is None
+    if packed:
+        if users.dtype != torch.int64:
+            raise TypeError("packed rating records must be an int64 tensor (see pack_ratings)")
+    else:
+        _req(items, "items"); _req(ratings, "ratings", torch.float32)
+        if users.dtype != items.dtype:
+            raise TypeError("users and items must share an integer dtype")
+        if items.numel() != users.numel() or ratings.numel() != users.numel():
+            raise ValueError("users, items and ratings must have the same length")
+    if int(neg_rate) < 0:
+        raise ValueError("neg_rate must be >= 0")
+    n, per, dev = users.numel(), 1 + int(neg_rate), users.device
+    out = (torch.empty(n * per, dtype=torch.int32, device=dev), torch.empty(n * per, dtype=torch.int32, device=dev),
+           torch.empty(n * per, dtype=torch.float32, device=dev))
+    a = NegDomainArgsC()
+    a.users = users.data_ptr()
+    a.items = None if packed else items.data_ptr()
+    a.ratings = None if packed else ratings.data_ptr()
+    a.n_pos = n; a.neg_rate = int(neg_rate); a.format = 1 if packed else 0
+    a.seed = seed & (2**64 - 1); a.step = int(step); a.max_tries = int(max_tries)
+    a.out_users, a.out_items, a.out_ratings = (t.data_ptr() for t in out)
+    return a, out, (4 if packed else _id_bytes(users))
+
+
+def seen_registry(num_items: int, device) -> tuple:
+    """Empty seen-items registry of :func:`neg_sample_seen` for ids ``[0, num_items)``: ``(order, count,
+    first_pos)`` = int32 ``[num_items]`` ids in first-occurrence order, int32 ``[1]`` how many, and int32
+    ``[num_items]`` per-item state (``-1`` registered, ``2**31 - 1`` not seen)."""
+    n = max(int(num_items), 1)
+    return (torch.zeros(n, dtype=torch.int32, device=device), torch.zeros(1, dtype=torch.int32, device=device),
+            torch.full((n,), 2**31 - 1, dtype=torch.int32, device=device))
+
+
+def neg_sample_seen(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Optional[torch.Tensor],
+                    neg_rate: int, registry: tuple, seen: Optional[torch.Tensor] = None,
+                    seen_pos: Optional[torch.Tensor] = None, user_div: int = 1, seed: int = 0, step: int = 0,
+                    max_tries: int = 32):
+    """:func:`neg_sample` with negatives drawn from the items this worker has seen so far
+    (PSOnlineMatrixFactorizationWorker.scala:61-88; csrc/fps_negatives.cu).  ``registry`` (from
+    :func:`seen_registry`) holds them in first-occurrence order and is advanced past the micro-batch in place.
+
+    Record ``p`` draws from ``D_p`` = the registry before the batch plus the batch's items first seen at
+    positions ``< p`` (its own first-seen item is not in its domain), ``max(0, min(|D_p| - |ring_p|, neg_rate))``
+    negatives, each uniform over ``D_p`` and none the positive or in the user's recent-items ring ``seen``
+    (``[n_local_users, userMemory]`` int32, updated in place as :func:`neg_sample` does; ``None`` = no ring,
+    ``|ring_p| = 0``).  Returns ``(users, items, ratings)`` int32/int32/float32 of length ``n*(1+neg_rate)``:
+    the positive, then its negatives; the slots not drawn, and draws that found nothing admissible in
+    ``max_tries`` tries, have user == -1.  ``items=None``: ``users`` holds packed64 records.  Item ids outside
+    ``[0, num_items)`` are never registered.  The output depends on ``seed``, ``step`` and the stream only."""
+    a, out, id_bytes = _neg_domain_args(users, items, ratings, neg_rate, seed, step, max_tries)
+    order, count, first_pos = registry
+    _req(order, "order", torch.int32); _req(count, "count", torch.int32); _req(first_pos, "first_pos", torch.int32)
+    if order.numel() != first_pos.numel():
+        raise ValueError("registry order and first_pos must have the same length")
+    if seen is not None:
+        _req(seen, "seen", torch.int32); _req(seen_pos, "seen_pos", torch.int32)
+        a.seen, a.seen_pos, a.memory = seen.data_ptr(), seen_pos.data_ptr(), int(seen.shape[1])
+    n, dev = users.numel(), users.device
+    cta_cap = sm_count(dev.index) * 8
+    scratch = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+    cta_new = torch.empty(cta_cap, dtype=torch.int32, device=dev)
+    a.user_div = int(user_div); a.cta_cap = cta_cap; a.num_items = order.numel()
+    a.order, a.count, a.first_pos = order.data_ptr(), count.data_ptr(), first_pos.data_ptr()
+    a.scratch, a.cta_new = scratch.data_ptr(), cta_new.data_ptr()
+    _check(lib().fps_neg_sample_seen(C.byref(a), id_bytes, sm_count(dev.index), _stream()), "neg_sample_seen")
+    _bump()
+    return out
+
+
+def noise_cdf(counts: torch.Tensor, power: float) -> torch.Tensor:
+    """fp64 inverse CDF ``cdf[i] = sum_{j <= i} w_j`` of the noise weights ``w = counts ** power`` (``w = 0``
+    where ``counts == 0``), built on the device by left-to-right sums, so a word of weight 0 has exactly its
+    predecessor's prefix.  ``counts``: float64 CUDA tensor of non-negative finite values."""
+    _req(counts, "counts", torch.float64)
+    n = counts.numel()
+    cdf = torch.empty(n, dtype=torch.float64, device=counts.device)
+    totals = torch.empty(-(-n // 256), dtype=torch.float64, device=counts.device)
+    _check(lib().fps_noise_cdf(C.c_void_p(counts.data_ptr()), C.c_longlong(n), C.c_double(float(power)),
+                               C.c_void_p(cdf.data_ptr()), C.c_void_p(totals.data_ptr()), _stream()), "noise_cdf")
+    _bump(3)
+    return cdf
+
+
+def neg_sample_noise(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Optional[torch.Tensor],
+                     neg_rate: int, cdf: torch.Tensor, last_nonzero: int, seed: int = 0, step: int = 0,
+                     max_tries: int = 32):
+    """:func:`neg_sample` with negatives drawn from fixed weights (skip-gram's unigram noise;
+    csrc/fps_negatives.cu): a 53-bit Philox uniform, scaled by the total weight, then an upper-bound binary
+    search of ``cdf`` (:func:`noise_cdf`), rejecting the positive ``items[p]``.  ``last_nonzero``: the last id
+    of positive weight.  Returns ``(users, items, ratings)`` int32/int32/float32 of length ``n*(1+neg_rate)``;
+    a negative that was the positive in all ``max_tries`` draws has user == -1.  Words of weight 0 are never
+    drawn.  ``items=None``: ``users`` holds packed64 records."""
+    a, out, id_bytes = _neg_domain_args(users, items, ratings, neg_rate, seed, step, max_tries)
+    _req(cdf, "cdf", torch.float64)
+    if not 0 <= int(last_nonzero) < cdf.numel():
+        raise ValueError("last_nonzero must index cdf")
+    a.cdf, a.vocab, a.last_nonzero = cdf.data_ptr(), cdf.numel(), int(last_nonzero)
+    _check(lib().fps_neg_sample_noise(C.byref(a), id_bytes, sm_count(users.device.index), _stream()),
+           "neg_sample_noise")
+    _bump()
+    return out
+
+
 class BucketArgsC(C.Structure):
     """Mirror of ``struct BucketArgs`` (csrc/fps_bucket.cu)."""
 
