@@ -199,6 +199,34 @@ def bpr_delta(u: Vector, vi: Vector, vj: Vector, lr: float, reg: float):
     return du, dvi, dvj, loss
 
 
+def warp_delta(u: Vector, vi: Vector, cand_rows, margin: float, lr: float, reg: float, rank_items: int):
+    """One WARP step (Weston, Bengio and Usunier 2011) for the positive ``(u, i)`` and its candidates in draw order,
+    ``cand_rows`` (``None`` = a void candidate: skipped, not counted); the reference of the device kernel
+    ``fps_mf_warp``.  The first live ``t*`` with ``x = u . (vi - v_t*) < margin`` violates; with ``n`` the live
+    candidates examined up to and including it, ``L = ln(max(1, (rank_items - 1) // n))`` and the deltas are those of
+    ``L * (margin - x) + reg/2 * (|u|^2 + |vi|^2 + |vj|^2)`` at fixed ``L``, all computed from the given values.
+
+    Returns ``(du, dvi, t*, dvj, n, L, loss)`` with ``loss = L * (margin - x)``; when no candidate violates (no
+    update) ``du``, ``dvi``, ``t*`` and ``dvj`` are ``None``, ``L`` and ``loss`` are 0 and ``n`` counts every live
+    candidate."""
+    u, vi = np.asarray(u, dtype=np.float64), np.asarray(vi, dtype=np.float64)
+    n = 0
+    for t, vj in enumerate(cand_rows):
+        if vj is None:
+            continue
+        n += 1
+        vj = np.asarray(vj, dtype=np.float64)
+        x = float(np.dot(u, vi - vj))
+        if x < margin:
+            L = math.log(max(1, (int(rank_items) - 1) // n))
+            g = lr * L
+            du = g * (vi - vj) - lr * reg * u
+            dvi = g * u - lr * reg * vi
+            dvj = -g * u - lr * reg * vj
+            return du, dvi, t, dvj, n, L, L * (margin - x)
+    return None, None, None, None, n, 0.0, 0.0
+
+
 def rowwise_adagrad(row: Vector, G: float, delta: Vector, lr: float, k: int, eps: float = 1e-8):
     """One row-wise AdaGrad step of a row whose learning-rate-1 SGD delta is ``delta`` and whose accumulator
     reads ``G``: ``s = |delta|^2 / k``, ``row + lr * delta / (sqrt(G + s) + eps)``.  Returns ``(new_row, s)``; the
@@ -213,6 +241,9 @@ def require_pointwise(backend: str, kw: dict) -> None:
     """The host tiers (``backend="local"`` / ``"native"``) train the pointwise loss with SGD only."""
     if backend != "device" and (kw.get("loss", "pointwise") != "pointwise" or kw.get("regularization", 0)):
         raise ValueError(f"loss={kw.get('loss')!r} / regularization need backend='device' "
+                         f"(backend={backend!r} trains the pointwise loss only)")
+    if backend != "device" and "margin" in kw:
+        raise ValueError(f"margin (of loss='warp') needs backend='device' "
                          f"(backend={backend!r} trains the pointwise loss only)")
     if backend != "device" and kw.get("optimizer", "sgd") != "sgd":
         raise ValueError(f"optimizer={kw.get('optimizer')!r} needs backend='device' "

@@ -16,6 +16,7 @@ with ``red.global.add.v4.f32`` -- no messages, no NCCL, no separate elementwise 
 """
 from __future__ import annotations
 
+import math
 import os
 from typing import Iterable, Optional, Sequence, Tuple
 
@@ -61,6 +62,27 @@ def check_optimizer(optimizer: str, *, item_cache: bool, output_ring=None, kerne
 
 
 NEGATIVE_SAMPLING = ("uniform", "seen")
+STATS_SIZE = {"pointwise": 2, "bpr": 3, "warp": 4}
+
+
+def check_warp(loss: str, margin: Optional[float], *, optimizer: str, negative_sampling: str) -> Optional[float]:
+    """The margin :class:`DeviceOnlineMF` trains ``loss`` with (``None`` unless ``loss="warp"``, whose default is
+    1.0); ``ValueError`` for a setting WARP cannot run.  WARP runs with SGD only, and its rank estimate needs one
+    candidate domain for every record: ``negative_sampling="uniform"``."""
+    if loss != "warp":
+        if margin is not None:
+            raise ValueError(f"margin is a parameter of loss='warp' (got loss={loss!r}): drop margin= or pass "
+                             f"loss='warp'")
+        return None
+    margin = 1.0 if margin is None else float(margin)
+    if not math.isfinite(margin):
+        raise ValueError(f"margin must be a finite number, got {margin!r}")
+    if optimizer != "sgd":
+        raise ValueError(f"loss='warp' trains with SGD only: pass optimizer='sgd' (got {optimizer!r})")
+    if negative_sampling != "uniform":
+        raise ValueError("loss='warp' needs negative_sampling='uniform': its rank estimate assumes every record "
+                         "draws from the same item range")
+    return margin
 
 
 def check_negative_sampling(negative_sampling: str, negative_sample_rate: int, negatives=None) -> None:
@@ -127,7 +149,7 @@ class DeviceOnlineMF:
                  flush_require: str = "any", replica_own_inplace: Optional[bool] = None,
                  output_ring=None, loss: str = "pointwise", regularization: float = 0.0,
                  step_window: Optional[int] = None, optimizer: str = "sgd",
-                 negative_sampling: str = "uniform"):
+                 negative_sampling: str = "uniform", margin: Optional[float] = None):
         """``loss="bpr"``: pairwise (Bayesian Personalised Ranking) updates, each positive rating paired
         with ``negative_sample_rate`` negatives (sampled) or with the ``negatives=`` of :meth:`step`;
         ``regularization`` is its L2 weight.  The pointwise loss has no regulariser.
@@ -145,23 +167,30 @@ class DeviceOnlineMF:
         has seen so far (DESIGN §2.11): a device registry keeps them in first-occurrence order (see
         :meth:`seen_items`), rating ``p`` of a micro-batch samples from the items seen before it, rejecting the
         user's last ``user_memory`` items and the positive, and gets ``min(negative_sample_rate, |domain| -
-        |user's recent items|)`` negatives.  It needs ``negative_sample_rate >= 1``."""
+        |user's recent items|)`` negatives.  It needs ``negative_sample_rate >= 1``.
+
+        ``loss="warp"``: WARP, the Weighted Approximate-Rank Pairwise loss (DESIGN §2.12).  Each positive rating
+        examines up to ``negative_sample_rate`` candidates (sampled as BPR's negatives, or the ``negatives=`` of
+        :meth:`step`) until one scores within ``margin`` (default 1.0) of the positive, and makes one hinge update
+        scaled by ``ln((num_items - 1) // n)``, ``n`` the candidates it took.  ``regularization`` is its L2 weight.  It
+        runs with SGD and ``negative_sampling="uniform"``, in the direct and the replica mode."""
         self._pending = []           # staged micro-batches of the step window: (records, format)
         self.step_window = 0
         check_negative_sampling(negative_sampling, negative_sample_rate)
         self.negative_sampling = negative_sampling
-        if loss not in ("pointwise", "bpr"):
-            raise ValueError(f"loss must be 'pointwise' or 'bpr', got {loss!r}")
+        if loss not in ("pointwise", "bpr", "warp"):
+            raise ValueError(f"loss must be 'pointwise', 'bpr' or 'warp', got {loss!r}")
         self.loss, self.reg = loss, float(regularization)
         if loss == "pointwise" and self.reg != 0.0:
-            raise ValueError("regularization is only supported with loss='bpr'")
-        if loss == "bpr":
+            raise ValueError("regularization is only supported with loss='bpr' or loss='warp'")
+        self.margin = check_warp(loss, margin, optimizer=optimizer, negative_sampling=negative_sampling)
+        if loss != "pointwise":
             if output_ring is not None:
-                raise ValueError("the per-update output ring is not supported with loss='bpr'")
+                raise ValueError(f"the per-update output ring is not supported with loss={loss!r}")
             if kernel == "tma":
-                raise ValueError("kernel='tma' is not supported with loss='bpr'")
+                raise ValueError(f"kernel='tma' is not supported with loss={loss!r}")
             if item_blocking:
-                raise ValueError("item_blocking is not supported with loss='bpr'")
+                raise ValueError(f"item_blocking is not supported with loss={loss!r}")
             item_blocking = False
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.cuda_device = torch.device("cuda", self.device)
@@ -201,8 +230,9 @@ class DeviceOnlineMF:
                                      device=self.cuda_device)
             native.init_rows(self._users, self.k, self.rank, self.world, native.PART_HASH, n_local,
                              seed * 2 + 2, range_min, range_max)
-            # pointwise: [sum (r - u.v)^2, updates]; BPR: [sum softplus(-x), triples, triples with x > 0]
-            self._stats = torch.zeros(3 if loss == "bpr" else 2, dtype=torch.float32, device=self.cuda_device)
+            # pointwise: [sum (r - u.v)^2, updates]; BPR: [sum softplus(-x), triples, triples with x > 0];
+            # WARP: [sum L * (margin - x), positives updated, candidates examined, positives]
+            self._stats = torch.zeros(STATS_SIZE[loss], dtype=torch.float32, device=self.cuda_device)
             # row-wise AdaGrad: one fp32 accumulator per user row (worker-local) and per item row (item shard)
             self._user_acc = self._item_acc = None
             if optimizer == "adagrad":
@@ -366,7 +396,8 @@ class DeviceOnlineMF:
              ratings: Optional[torch.Tensor] = None, negatives: Optional[torch.Tensor] = None) -> None:
         """Process one micro-batch of ratings whose users belong to this worker (async SGD).
         ``step(packed)`` with a single int64 tensor takes packed64 records (``native.pack_ratings``).
-        ``negatives`` (``loss="bpr"`` only): ``[n, m]`` item ids paired with each rating, ``-1`` = none.
+        ``negatives`` (``loss="bpr"`` / ``"warp"`` only): ``[n, m]`` item ids paired with each rating, ``-1`` = none
+        (WARP: the candidates, examined in column order).
 
         Lazy with a step window (``step_window``): an eligible micro-batch (:func:`step_windowable`) is only
         copied into a device staging slot -- the caller may reuse its tensors at once -- and the window is
@@ -382,11 +413,11 @@ class DeviceOnlineMF:
             return
         self._drain()
         check_negative_sampling(self.negative_sampling, self.neg, negatives)
-        if self.loss == "bpr":
-            self._step_bpr(users, items, ratings, negatives)
+        if self.loss != "pointwise":
+            self._step_pairwise(users, items, ratings, negatives)
             return
         if negatives is not None:
-            raise ValueError("negatives= needs loss='bpr'")
+            raise ValueError("negatives= needs loss='bpr' or loss='warp'")
         neg = self.neg
         if self.user_memory > 0 or self._registry is not None:
             # negatives drawn by a sampler kernel (the per-user seen ring, the seen-items registry); the fused kernel
@@ -434,13 +465,13 @@ class DeviceOnlineMF:
         self.step_no += 1
         METRICS.inc("mf_ratings", users.numel())
 
-    def _step_bpr(self, users, items, ratings, negatives) -> None:
+    def _step_pairwise(self, users, items, ratings, negatives) -> None:
         if negatives is not None:
             if self.item_cache:
                 raise ValueError("negatives= is not supported in the replica (item_cache) mode")
             n = int(negatives.shape[1]) if negatives.dim() == 2 else 0
         elif self.neg < 1:
-            raise ValueError("loss='bpr' needs negative_sample_rate >= 1 or explicit negatives=")
+            raise ValueError(f"loss={self.loss!r} needs negative_sample_rate >= 1 or explicit negatives=")
         elif self.user_memory > 0 or self._registry is not None:
             # negatives that avoid the user's recent items: the sampler's expanded [n, 1 + m] records,
             # with the negatives it could not find voided
@@ -453,13 +484,22 @@ class DeviceOnlineMF:
         else:
             n = self.neg                   # drawn inside the kernel
         if self.output_ring is not None:
-            raise ValueError("the per-update output ring is not supported with loss='bpr'")
+            raise ValueError(f"the per-update output ring is not supported with loss={self.loss!r}")
         n_pos = users.numel()
         cand, reserve = self._items.table_c, 0
         if self.item_cache:
-            # uniform per-destination counts feed the flush policy (BPR batches are not dealt into buckets)
-            self.replica.after_step(n_pos * n, fed=False)
+            # uniform per-destination counts feed the flush policy (pairwise batches are not dealt into buckets);
+            # a WARP positive updates at most one candidate
+            self.replica.after_step(n_pos * (n if self.loss == "bpr" else 1), fed=False)
             cand, reserve = self.replica.table_c, self.replica.reserve_total()
+        if self.loss == "warp":
+            native.mf_warp_fused(users, items, ratings, self._users, cand, self.lr, self.reg, margin=self.margin,
+                                 rank_items=self.num_items, negatives=negatives, n_neg=n, num_items=self.num_items,
+                                 seed=self.seed, step=self.step_no, anchor_div=self.world, stats=self._stats,
+                                 nan_flag=self._nan_flag, max_inflight_rows=self.pull_limit, reserve_total=reserve)
+            self.step_no += 1
+            METRICS.inc("mf_ratings", n_pos)
+            return
         native.mf_bpr_fused(users, items, ratings, self._users, cand, self.lr, self.reg, negatives=negatives,
                             n_neg=n, num_items=self.num_items, seed=self.seed, step=self.step_no,
                             anchor_div=self.world, stats=self._stats, nan_flag=self._nan_flag,
@@ -528,7 +568,8 @@ class DeviceOnlineMF:
 
         Yields one host-side ``(sum_sq_err, n_updates)`` per micro-batch (device -> host read of
         the step's result), lagging the launch by one step so copies, kernels and reads overlap.
-        With ``loss="bpr"`` the pair is ``(sum softplus(-x), n_triples)``.
+        With ``loss="bpr"`` the pair is ``(sum softplus(-x), n_triples)``, with ``loss="warp"`` ``(sum L * (margin -
+        x), positives updated)``.
         It reads the loss after every micro-batch, so it takes the per-launch path (no step window).
         """
         self._drain()

@@ -17,7 +17,7 @@ from ...api import Left, Right
 from ...ops import native
 from ...runtime.stream import ResultStream, as_stream
 from .common import Rating
-from .device import ERR_PLAIN, ERR_SIGMOID, DeviceOnlineMF
+from .device import ERR_PLAIN, ERR_SIGMOID, STATS_SIZE, DeviceOnlineMF, check_warp
 
 
 def _batches(src, batch_size: int) -> Iterator[Sequence[torch.Tensor]]:
@@ -74,20 +74,23 @@ def ps_online_mf_device(src, numFactors=10, rangeMin=-0.01, rangeMax=0.01, learn
                         userMemory: int = 128, updateOutput: Optional[int] = None,
                         outputFlushCount: int = 1, outputFlushMs: Optional[float] = None,
                         loss: str = "pointwise", regularization: float = 0.0,
-                        optimizer: str = "sgd", negativeSampling: Optional[str] = None) -> ResultStream:
+                        optimizer: str = "sgd", negativeSampling: Optional[str] = None,
+                        margin: Optional[float] = None) -> ResultStream:
     """``updateOutput=n``: also emit ``Left((userId, userVector))`` for one update in ``n`` (``1`` = every
     update, the reference's worker output PSOnlineMatrixFactorizationWorker.scala:52) through the device
     output ring (count / timer flushed on the device); the final dump then holds only the item shard.
     ``loss="bpr"``: pairwise updates, every rating > 0 paired with ``negativeSampleRate`` sampled
     negatives, L2 weight ``regularization`` (see :class:`DeviceOnlineMF`); it has no per-update output,
     so ``updateOutput`` with ``loss="bpr"`` raises ``ValueError``.
+    ``loss="warp"``: WARP, each rating > 0 examining up to ``negativeSampleRate`` sampled candidates until one is
+    within ``margin`` (default 1.0) of it (see :class:`DeviceOnlineMF`); no per-update output either.
     ``optimizer="adagrad"``: row-wise AdaGrad (see :class:`DeviceOnlineMF`); a multi-rank job then reads and
     updates the item rows on their owners (no item cache).
     ``negativeSampling="seen"``: negatives from the items each rank has seen so far, the rule of the reference and
     the host tiers (see :class:`DeviceOnlineMF`); the registry of seen items carries over from epoch to epoch.
     ``None`` or ``"uniform"``: uniform over the whole item range."""
     if updateOutput and loss != "pointwise":
-        raise ValueError("updateOutput (the per-update output ring) is not supported with loss='bpr'")
+        raise ValueError(f"updateOutput (the per-update output ring) is not supported with loss={loss!r}")
     recs = None
     if numUsers is None or numItems is None:
         recs = list(src.collect() if hasattr(src, "collect") else src)
@@ -105,7 +108,7 @@ def ps_online_mf_device(src, numFactors=10, rangeMin=-0.01, rangeMax=0.01, learn
                            user_memory=min(int(userMemory), 256) if negativeSampleRate > 0 else 0,
                            loss=loss, regularization=regularization, optimizer=optimizer,
                            item_cache=False if optimizer == "adagrad" else None,
-                           negative_sampling=negativeSampling or "uniform")
+                           negative_sampling=negativeSampling or "uniform", margin=margin)
     ring, updates = None, []
     if updateOutput:
         from ...runtime.output_ring import OutputRing
@@ -297,7 +300,7 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
                                            K=100, workerK=None, pullLimit=0, seed=0, plain_residual=False,
                                            numUsers: Optional[int] = None, numItems: Optional[int] = None,
                                            batch_size: int = 4096, group=None, loss: str = "pointwise",
-                                           regularization: float = 0.0):
+                                           regularization: float = 0.0, margin: Optional[float] = None):
     """Online MF plus a top-K list for every incoming rating, computed BEFORE the model sees that rating
     (prequential evaluation; ``psOnlineLearnerAndGenerator``,
     PSOnlineMatrixFactorizationAndTopKGenerator.scala:51-101) on the device tier, any number of ranks.
@@ -315,6 +318,10 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
        pushed to the PS (``...AndTopKGeneratorWorker.scala:128-164``) -- the fused MF kernel with the
        roles swapped (worker-local rows = items, PS rows = users), negatives drawn from the owner's items.
 
+    ``loss="warp"``: the owner examines its ``[n, negativeSampleRate]`` candidate draws in order until one is
+    within ``margin`` (default 1.0) of the positive; the rank estimate uses ``numItems`` (the owner's items are a
+    uniform subset of all items, so ``(numItems - 1) / n`` still estimates the global rank).
+
     Prequential at micro-batch granularity (``batch_size``; 1 reproduces the per-rating order).  The
     result is a pure function of the stream and the seed, whatever the number of ranks (init is Philox
     by id).  Rank 0 returns ``[(userId, itemId, timestamp, [(score, itemId)])]`` (other ranks ``[]``);
@@ -325,12 +332,13 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
     from ...store.sharded_table import ShardedTable
     from .device_topk import DeviceTopK, DistributedTopK
 
-    if loss not in ("pointwise", "bpr"):
-        raise ValueError(f"loss must be 'pointwise' or 'bpr', got {loss!r}")
+    if loss not in ("pointwise", "bpr", "warp"):
+        raise ValueError(f"loss must be 'pointwise', 'bpr' or 'warp', got {loss!r}")
     if loss == "pointwise" and regularization != 0:
-        raise ValueError("regularization is only supported with loss='bpr'")
-    if loss == "bpr" and negativeSampleRate < 1:
-        raise ValueError("loss='bpr' needs negativeSampleRate >= 1")
+        raise ValueError("regularization is only supported with loss='bpr' or loss='warp'")
+    if loss != "pointwise" and negativeSampleRate < 1:
+        raise ValueError(f"loss={loss!r} needs negativeSampleRate >= 1")
+    margin = check_warp(loss, margin, optimizer="sgd", negative_sampling="uniform")
     recs = list(src.collect() if hasattr(src, "collect") else src)
     if numUsers is None:
         numUsers = 1 + max((r.user for r in recs), default=0)
@@ -348,7 +356,7 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
     native.init_rows(items, numFactors, rank, world, native.PART_HASH, n_local, seed * 2 + 1, rangeMin, rangeMax)
     local_ids = torch.arange(n_local, device=dev, dtype=torch.int64) * world + rank
     n_valid = int((local_ids < numItems).sum())
-    stats = torch.zeros(3 if loss == "bpr" else 2, dtype=torch.float32, device=dev)
+    stats = torch.zeros(STATS_SIZE[loss], dtype=torch.float32, device=dev)
     nan_flag = torch.zeros(1, dtype=torch.int32, device=dev)
     err_mode = ERR_PLAIN if plain_residual else ERR_SIGMOID
     wk = max(workerK or K, K)
@@ -395,6 +403,11 @@ def ps_online_learner_and_generator_device(src, numFactors=10, rangeMin=-0.001, 
                 native.mf_bpr_fused(u, ti, rt, users.table_c, items, learningRate, regularization,
                                     negatives=neg_item.contiguous(), cand_div=world, stats=stats,
                                     nan_flag=nan_flag, max_inflight_rows=int(pullLimit or 0))
+        elif loss == "warp":
+            if n_valid > 0:
+                native.mf_warp_fused(u, ti, rt, users.table_c, items, learningRate, regularization, margin=margin,
+                                     rank_items=numItems, negatives=neg_item.contiguous(), cand_div=world,
+                                     stats=stats, nan_flag=nan_flag, max_inflight_rows=int(pullLimit or 0))
         else:
             native.mf_sgd_fused(ti.contiguous(), tu.contiguous(), tr.contiguous(), items, world, users.table_c,
                                 learningRate, err_mode=err_mode, stats=stats, nan_flag=nan_flag,

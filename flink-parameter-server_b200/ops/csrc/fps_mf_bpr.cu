@@ -29,52 +29,7 @@
 #include "fps_common.cuh"
 #include "fps_mf_args.cuh"
 
-struct BprArgs {
-  const void* users;          // anchor ids, or packed64 records (user:26 | item:22 | rating fp16:16)
-  const void* items;          // positive candidate ids
-  const float* ratings;       // records with rating <= 0 are skipped
-  const void* negatives;      // [n_pos, n_neg] candidate ids, -1 = void; nullptr = sampled in the kernel
-  long long n_pos;
-  int n_neg;
-  int format;                 // 0: users/items/ratings arrays; 1: packed64 records in `users`
-  long long num_items;        // sampled negatives: id range [0, num_items)
-  unsigned long long seed;    // sampled negatives: stream key
-  unsigned long long step;    // sampled negatives: stream counter (micro-batch number)
-  float lr;
-  float reg;
-  float* anchor_table;        // worker-local [rows, stride] when anchor_sharded == 0
-  int anchor_div;             //   slot = id / anchor_div
-  int anchor_shift;           //   log2(anchor_div) if a power of two, else -1
-  int anchor_sharded;         // != 0: anchor rows are read and pushed through anchor_tab
-  int cand_sharded;           // != 0: candidate rows are read through cand_tab
-  ShardTable anchor_tab;
-  float* cand_table;          // worker-local [rows, stride] when cand_sharded == 0
-  int cand_div;
-  int cand_shift;
-  ShardTable cand_tab;
-  int use_push_tab;           // != 0 (with cand_sharded): candidate deltas go to push_tab
-  int stride;                 // row stride in floats, shared by every table
-  ShardTable push_tab;
-  float* stats;               // [0] += softplus(-x), [1] += #triples, [2] += #(x > 0)
-  int* nan_flag;              // set to 1 if a non-finite update was produced
-  int reserve_total;          // CTA slots left free on the whole GPU (the replica exchange CTAs)
-  int pad_;
-  // Row-wise AdaGrad accumulators (one fp32 per row, stride 1); cand_acc.base[0] == nullptr means SGD
-  ShardTable anchor_acc_tab;  // anchor accumulators when anchor_sharded != 0
-  ShardTable cand_acc;        // candidate accumulators, addressed like cand_tab
-  float* anchor_acc;          // worker-local anchor accumulators (slot = id / anchor_div) otherwise
-};
-
-template <typename IdT>
-__device__ __forceinline__ float* bpr_row(float* local, int div, int shift, int sharded,
-                                          const ShardTable& t, IdT id, int stride) {
-  if (sharded) return fps_row_t<IdT>(t, id);
-  return local + fps_user_slot<IdT>(id, div, shift) * (size_t)stride;
-}
-
-__device__ __forceinline__ float4 bpr_axpy(float a, float4 x, float b, float4 y) {
-  return make_float4(a * x.x + b * y.x, a * x.y + b * y.y, a * x.z + b * y.z, a * x.w + b * y.w);
-}
+// BprArgs, bpr_row and bpr_axpy: fps_mf_args.cuh (shared with the WARP step of fps_mf_warp.cu)
 
 template <typename IdT, int LPR, int VPL, int MINB, int FMT>
 __global__ void __launch_bounds__(256, MINB) fps_mf_bpr_kernel(const __grid_constant__ BprArgs a) {

@@ -7,6 +7,7 @@ no PyTorch fallback on a GPU box: if the library is missing the ops raise.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import threading
 from typing import Optional
@@ -398,7 +399,7 @@ def mf_window_drain(stage: torch.Tensor, slot_bytes: int, counts, formats, user_
 
 
 class BprArgsC(C.Structure):
-    """Mirror of ``struct BprArgs`` (csrc/fps_mf_bpr.cu)."""
+    """Mirror of ``struct BprArgs`` (csrc/fps_mf_args.cuh)."""
 
     _fields_ = [
         ("users", C.c_void_p), ("items", C.c_void_p), ("ratings", C.c_void_p), ("negatives", C.c_void_p),
@@ -411,35 +412,14 @@ class BprArgsC(C.Structure):
         ("use_push_tab", C.c_int), ("stride", C.c_int), ("push_tab", ShardTableC),
         ("stats", C.c_void_p), ("nan_flag", C.c_void_p), ("reserve_total", C.c_int), ("pad_", C.c_int),
         ("anchor_acc_tab", ShardTableC), ("cand_acc", ShardTableC), ("anchor_acc", C.c_void_p),
+        ("rank_items", C.c_longlong), ("margin", C.c_float), ("pad2_", C.c_int),
     ]
 
 
-def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Optional[torch.Tensor],
-                 anchor_table, cand_table, lr: float, reg: float = 0.0, *,
-                 negatives: Optional[torch.Tensor] = None, n_neg: int = 1, num_items: int = 0,
-                 seed: int = 0, step: int = 0, anchor_div: int = 1, cand_div: int = 1,
-                 stats: Optional[torch.Tensor] = None, nan_flag: Optional[torch.Tensor] = None,
-                 max_inflight_rows: int = 0, push_tab: Optional[ShardTableC] = None,
-                 reserve_total: int = 0, anchor_acc=None, cand_acc: Optional[ShardTableC] = None) -> None:
-    """Fused pairwise (BPR) pull + SGD + push, one ``(anchor, positive, negative)`` triple per update
-    (csrc/fps_mf_bpr.cu).  ``users`` are the anchor ids, ``items`` the positive candidates; records with
-    ``rating <= 0`` are skipped.  ``items=None``: ``users`` holds packed64 records (:func:`pack_ratings`).
-
-    ``anchor_table`` / ``cand_table``: a worker-local ``[rows, stride]`` float32 tensor (row of id =
-    ``id // anchor_div`` / ``id // cand_div``) or a :class:`ShardTableC`.  ``push_tab`` (with a
-    ShardTable ``cand_table``) receives the candidate deltas instead of ``cand_table``.
-
-    ``negatives``: ``[n_pos, n]`` ids of the same dtype as ``users`` (int32 for packed64), ``-1`` voids a
-    triple.  Without it ``n_neg`` negatives per positive are drawn in the kernel, uniform over
-    ``[0, num_items)`` and never the positive.  ``stats`` (float32 ``[3]``) accumulates the softplus loss
-    sum, the number of triples and the number with ``x > 0``.  ``max_inflight_rows`` caps the grid so that
-    at most that many rows are being pulled at once (3 per lane-group).  ``reserve_total``: CTA slots
-    the grid leaves free for a kernel running next to it (the replica exchange).
-
-    ``cand_acc`` / ``anchor_acc``: row-wise AdaGrad instead of SGD (DESIGN §2.10).  ``cand_acc`` is a stride-1
-    :class:`ShardTableC` of candidate accumulators (``cand_table`` must then be a ShardTableC, without
-    ``push_tab``); ``anchor_acc`` a float32 ``[rows]`` tensor, or a stride-1 ShardTableC when ``anchor_table``
-    is one."""
+def _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, negatives, n_neg, num_items, seed,
+                   step, anchor_div, cand_div, stats, n_stats, nan_flag, push_tab, reserve_total):
+    """The validated :class:`BprArgsC` of :func:`mf_bpr_fused` / :func:`mf_warp_fused`, and whether ``users`` holds
+    packed64 records."""
     _req(users, "users")
     packed = items is None
     if packed:
@@ -485,8 +465,8 @@ def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Op
         a.n_neg = int(n_neg)
     if stats is not None:
         _req(stats, "stats", torch.float32)
-        if stats.numel() < 3:
-            raise ValueError("stats must hold 3 floats")
+        if stats.numel() < n_stats:
+            raise ValueError(f"stats must hold {n_stats} floats")
         a.stats = stats.data_ptr()
     if nan_flag is not None:
         _req(nan_flag, "nan_flag", torch.int32)
@@ -498,6 +478,37 @@ def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Op
     a.n_pos = n_pos; a.num_items = int(max(num_items, 1))
     a.seed = seed & (2**64 - 1); a.step = int(step)
     a.lr = float(lr); a.reg = float(reg); a.reserve_total = int(reserve_total)
+    return a, packed
+
+
+def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Optional[torch.Tensor],
+                 anchor_table, cand_table, lr: float, reg: float = 0.0, *,
+                 negatives: Optional[torch.Tensor] = None, n_neg: int = 1, num_items: int = 0,
+                 seed: int = 0, step: int = 0, anchor_div: int = 1, cand_div: int = 1,
+                 stats: Optional[torch.Tensor] = None, nan_flag: Optional[torch.Tensor] = None,
+                 max_inflight_rows: int = 0, push_tab: Optional[ShardTableC] = None,
+                 reserve_total: int = 0, anchor_acc=None, cand_acc: Optional[ShardTableC] = None) -> None:
+    """Fused pairwise (BPR) pull + SGD + push, one ``(anchor, positive, negative)`` triple per update
+    (csrc/fps_mf_bpr.cu).  ``users`` are the anchor ids, ``items`` the positive candidates; records with
+    ``rating <= 0`` are skipped.  ``items=None``: ``users`` holds packed64 records (:func:`pack_ratings`).
+
+    ``anchor_table`` / ``cand_table``: a worker-local ``[rows, stride]`` float32 tensor (row of id =
+    ``id // anchor_div`` / ``id // cand_div``) or a :class:`ShardTableC`.  ``push_tab`` (with a
+    ShardTable ``cand_table``) receives the candidate deltas instead of ``cand_table``.
+
+    ``negatives``: ``[n_pos, n]`` ids of the same dtype as ``users`` (int32 for packed64), ``-1`` voids a
+    triple.  Without it ``n_neg`` negatives per positive are drawn in the kernel, uniform over
+    ``[0, num_items)`` and never the positive.  ``stats`` (float32 ``[3]``) accumulates the softplus loss
+    sum, the number of triples and the number with ``x > 0``.  ``max_inflight_rows`` caps the grid so that
+    at most that many rows are being pulled at once (3 per lane-group).  ``reserve_total``: CTA slots
+    the grid leaves free for a kernel running next to it (the replica exchange).
+
+    ``cand_acc`` / ``anchor_acc``: row-wise AdaGrad instead of SGD (DESIGN §2.10).  ``cand_acc`` is a stride-1
+    :class:`ShardTableC` of candidate accumulators (``cand_table`` must then be a ShardTableC, without
+    ``push_tab``); ``anchor_acc`` a float32 ``[rows]`` tensor, or a stride-1 ShardTableC when ``anchor_table``
+    is one."""
+    a, packed = _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, negatives, n_neg, num_items,
+                               seed, step, anchor_div, cand_div, stats, 3, nan_flag, push_tab, reserve_total)
     if cand_acc is not None:
         if not a.cand_sharded or push_tab is not None:
             raise ValueError("row-wise AdaGrad needs a ShardTableC cand_table and no push_tab")
@@ -519,6 +530,41 @@ def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Op
         raise ValueError("anchor_acc needs cand_acc")
     _check(lib().fps_mf_bpr_fused(C.byref(a), 4 if packed else _id_bytes(users), int(max_inflight_rows),
                                   sm_count(users.device.index), _stream()), "mf_bpr_fused")
+    _bump()
+
+
+WARP_TRIAL_BLOCKS = (1, 2, 4, 8)   # candidates a lane-group pulls at once in fps_mf_warp (0 = per-geometry default)
+
+
+def mf_warp_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Optional[torch.Tensor],
+                  anchor_table, cand_table, lr: float, reg: float = 0.0, *, margin: float = 1.0,
+                  rank_items: int = 0, negatives: Optional[torch.Tensor] = None, n_neg: int = 1,
+                  num_items: int = 0, seed: int = 0, step: int = 0, anchor_div: int = 1, cand_div: int = 1,
+                  stats: Optional[torch.Tensor] = None, nan_flag: Optional[torch.Tensor] = None,
+                  max_inflight_rows: int = 0, push_tab: Optional[ShardTableC] = None, reserve_total: int = 0,
+                  trial_block: int = 0) -> None:
+    """Fused WARP (Weighted Approximate-Rank Pairwise) step (csrc/fps_mf_warp.cu, DESIGN §2.12): for each positive
+    ``(anchor, item)`` with ``rating > 0``, its candidates are examined in order until one violates
+    ``u . (v_i - v_j) < margin``; with ``n`` the live candidates examined up to it, the triple gets one hinge update
+    with ``g = lr * ln(max(1, (rank_items - 1) // n))``.  No violator: nothing is written.  The arguments are those
+    of :func:`mf_bpr_fused`: ``negatives`` ``[n_pos, T]`` are the candidates in order (``-1`` or the positive = void),
+    else ``T = n_neg`` are drawn in the kernel, candidate ``t`` bitwise BPR's negative ``t``.
+
+    ``rank_items``: the ``N`` of the rank estimate (``0`` = ``num_items``).  ``stats`` (float32 ``[4]``) accumulates
+    ``sum L * (margin - x)`` over the updated positives, the positives updated, the live candidates examined and the
+    positives considered.  ``max_inflight_rows`` caps the grid at ``2 + trial_block`` rows per lane-group.
+    ``trial_block`` (one of :data:`WARP_TRIAL_BLOCKS`, ``0`` = the default of the row width) changes the speed only:
+    the result is bitwise the same for all."""
+    if not math.isfinite(float(margin)):
+        raise ValueError(f"margin must be finite, got {margin!r}")
+    if int(trial_block) not in (0,) + WARP_TRIAL_BLOCKS:
+        raise ValueError(f"trial_block must be 0 or one of {WARP_TRIAL_BLOCKS}, got {trial_block!r}")
+    a, packed = _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, negatives, n_neg, num_items,
+                               seed, step, anchor_div, cand_div, stats, 4, nan_flag, push_tab, reserve_total)
+    a.margin = float(margin)
+    a.rank_items = int(rank_items) if int(rank_items) > 0 else int(a.num_items)
+    _check(lib().fps_mf_warp_fused(C.byref(a), 4 if packed else _id_bytes(users), int(trial_block),
+                                   int(max_inflight_rows), sm_count(users.device.index), _stream()), "mf_warp_fused")
     _bump()
 
 
