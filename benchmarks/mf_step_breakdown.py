@@ -16,7 +16,9 @@ Records, in one process:
 ``--window`` records the step window instead (``DeviceOnlineMF(step_window=8)``, fps_mf_window.cu), written to
 ``profiles/h100_mf_step_window.json`` by default: device times of the staging copies and of the drain for each
 kernel variant (CUDA events and ``torch.profiler``), the bytes model of a windowed step next to them, TB/s against
-the ``copy_`` ceiling, and A/B rows of the windowed and the per-launch step alternated round by round.
+the ``copy_`` ceiling, the drain's split into its build phase (scatter rounds) and its apply phase (chains) from
+the kernel's own ``%globaltimer`` marks, and A/B rows of the windowed and the per-launch step alternated round by
+round.
 """
 from __future__ import annotations
 
@@ -171,7 +173,8 @@ def bytes_model(n_per_mb, row_bytes, record_bytes, sort_pass_bytes):
     }
 
 
-WINDOW_VARIANTS = {"p4_3cta": "0", "p8_2cta": "1"}   # FPS_MF_WINDOW_VARIANT: user rows prefetched, CTAs/SM
+# FPS_MF_WINDOW_VARIANT at k = 64: (float4 per lane, user rows prefetched, CTAs/SM); see dispatch_window
+WINDOW_VARIANTS = {"v4_p2_2cta": "0", "v1_p4_3cta": "2", "v1_p8_2cta": "1"}
 
 
 def window_bytes_model(step, row_bytes):
@@ -188,17 +191,21 @@ def window_bytes_model(step, row_bytes):
             "staging_copy_bytes": staging, "drain_record_bytes": drain_records, "slot_table_bytes": slot_table,
             "user_rows_bytes": users, "item_rows_bytes": items,
             "drain_bytes": users + items + drain_records + slot_table,
+            "chain_bytes": users + items + 2 * 8 * n,   # rows, and each T entry read and reset by the chain
             "per_launch_bytes": 2 * row_bytes * n * 2 + 8 * n,
             "note": "computed from shapes and the step's item ids; slot-table and bitmap traffic are upper bounds "
                     "(they may be served by L2)"}
 
 
 def window_split(model, steps, n_steps):
-    """Device time of the staging copies and of the drain of each step, separately (CUDA events)."""
+    """Device time of the staging copies and of the drain of each step, separately (CUDA events), and the drain's
+    build and apply phases (the kernel's %globaltimer marks, CTA 0 after each grid sync)."""
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-    stage_ms, drain_ms = [], []
+    stage_ms, drain_ms, build_ms, apply_ms = [], [], [], []
+    model._win_phase_ns = torch.zeros(4, dtype=torch.int64, device=model.cuda_device)
     for s in range(n_steps):
         model.stats.zero_()
+        model._win_phase_ns.zero_()
         ev[0].record()
         for b in steps[s % len(steps)]:
             model._stage(b, None, None)
@@ -208,7 +215,12 @@ def window_split(model, steps, n_steps):
         torch.cuda.synchronize()
         stage_ms.append(ev[0].elapsed_time(ev[1]))
         drain_ms.append(ev[1].elapsed_time(ev[2]))
-    return statistics.median(stage_ms), statistics.median(drain_ms)
+        ph = model._win_phase_ns.tolist()
+        build_ms.append(ph[0] * 1e-6)
+        apply_ms.append(ph[1] * 1e-6)
+    model._win_phase_ns = None
+    return (statistics.median(stage_ms), statistics.median(drain_ms), statistics.median(build_ms),
+            statistics.median(apply_ms))
 
 
 def window_main(a, res, steps, sizes, DeviceOnlineMF):
@@ -226,10 +238,12 @@ def window_main(a, res, steps, sizes, DeviceOnlineMF):
         timed(m, steps, a.warmup, 0)
     for v, code in WINDOW_VARIANTS.items():
         os.environ["FPS_MF_WINDOW_VARIANT"] = code
-        stage, drain = window_split(win, steps, a.steps)
+        stage, drain, build, chain = window_split(win, steps, a.steps)
         prof = profile(win, steps, 4)
         res["window"]["variants"][v] = {
             "staging_ms_per_step": stage, "drain_ms_per_step": drain,
+            "build_ms_per_step": build, "chain_ms_per_step": chain,
+            "chain_tb_per_s": bm["chain_bytes"] / (chain * 1e-3) / 1e12,
             "drain_tb_per_s": bm["drain_bytes"] / (drain * 1e-3) / 1e12,
             "drain_share_of_copy_ceiling": bm["drain_bytes"] / (drain * 1e-3) / 1e12 / ceiling,
             "staging_tb_per_s": bm["staging_copy_bytes"] / (stage * 1e-3) / 1e12,

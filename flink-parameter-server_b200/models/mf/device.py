@@ -294,6 +294,7 @@ class DeviceOnlineMF:
                                             loss=self.loss, table_rows=self.num_items, stride=self._items.stride,
                                             env=os.environ.get("FPS_STEP_WINDOW"), optimizer=optimizer)
         self._win = None
+        self._win_phase_ns = None   # optional int64 [4]: build / apply ns of every drain (mf_window_drain)
         self._graph_capture = False
         self._per_launch = False
         self._items.barrier()
@@ -381,7 +382,7 @@ class DeviceOnlineMF:
         w = self._win
         native.mf_window_drain(w["stage"], w["slot_bytes"], counts, fmts, self._users, self._items.local, self.lr,
                                self.err_mode, w["slots"], w["user_bits"], w["ctl"], self._stats, w["slot_stats"],
-                               self._nan_flag)
+                               self._nan_flag, phase_ns=self._win_phase_ns)
         return n
 
     # ------------------------------------------------------------------------------------

@@ -355,20 +355,23 @@ class WinArgsC(C.Structure):
         ("user_table", C.c_void_p), ("item_table", C.c_void_p), ("rows", C.c_longlong),
         ("slots", C.c_void_p), ("user_bits", C.c_void_p), ("bm_words", C.c_longlong),
         ("ctl", C.c_void_p), ("stats", C.c_void_p), ("slot_stats", C.c_void_p), ("nan_flag", C.c_void_p),
+        ("phase_ns", C.c_void_p),
     ]
 
 
 def mf_window_drain(stage: torch.Tensor, slot_bytes: int, counts, formats, user_table: torch.Tensor,
                     item_table: torch.Tensor, lr: float, err_mode: int, slots: torch.Tensor,
                     user_bits: torch.Tensor, ctl: torch.Tensor, stats: torch.Tensor, slot_stats: torch.Tensor,
-                    nan_flag: torch.Tensor) -> None:
+                    nan_flag: torch.Tensor, phase_ns: Optional[torch.Tensor] = None) -> None:
     """Apply the micro-batches staged in ``stage`` (slot j at byte ``j * slot_bytes``: ``counts[j]`` records,
     ``formats[j]`` 1 = packed64, 0 = int32 users | int32 items | fp32 ratings) in order, in one cooperative
     launch (csrc/fps_mf_window.cu).  Conflict-free runs of micro-batches are applied item-major with the tables
     bitwise equal to one :func:`mf_sgd_fused` launch per micro-batch.  ``slots``: int64 ``[>= n, rows]``
     filled with -1, left so; ``user_bits``: int32 bitmap over the user rows; ``ctl``: int32 ``[2 * WINDOW_MAX]``;
     ``slot_stats``: float32 ``[>= n, 2]`` receives each micro-batch's (sum sq err, updates), ``stats`` the totals
-    (``DeviceOnlineMF`` reads only the totals; the per-micro-batch sums serve callers that report per micro-batch)."""
+    (``DeviceOnlineMF`` reads only the totals; the per-micro-batch sums serve callers that report per micro-batch).
+    ``phase_ns``: optional int64 ``[4]``; the drain adds its build and apply nanoseconds to ``[0]`` and ``[1]`` and
+    the windows it applied to ``[2]`` (``[3]`` is scratch)."""
     n = len(counts)
     if not 0 < n <= WINDOW_MAX or len(formats) != n:
         raise ValueError(f"1..{WINDOW_MAX} staged micro-batches expected, got {n}")
@@ -391,6 +394,11 @@ def mf_window_drain(stage: torch.Tensor, slot_bytes: int, counts, formats, user_
     a.slots = slots.data_ptr(); a.user_bits = user_bits.data_ptr(); a.bm_words = user_bits.numel()
     a.ctl = ctl.data_ptr(); a.stats = stats.data_ptr(); a.slot_stats = slot_stats.data_ptr()
     a.nan_flag = nan_flag.data_ptr()
+    if phase_ns is not None:
+        _req(phase_ns, "phase_ns", torch.int64)
+        if phase_ns.numel() < 4:
+            raise ValueError("phase_ns too small")
+        a.phase_ns = phase_ns.data_ptr()
     rv = os.environ.get("FPS_MF_WINDOW_VARIANT")
     if rv is not None:
         lib().fps_set_mf_window_variant(int(rv))
