@@ -11,6 +11,9 @@ label 0.  Not part of the reference's algorithm suite; it exercises the same API
 ``optimizer="adagrad"`` replaces the global rate by row-wise AdaGrad (DESIGN §2.10), with one fp32
 accumulator per row of each table on that row's shard.  ``noise_counts`` draws the negatives from the unigram
 noise ``counts ** noise_power`` (Mikolov et al. 2013) instead (DESIGN §2.11).
+``train_tokens`` / ``fit_tokens`` train from a token stream (DESIGN §2.13): frequent-word subsampling, dynamic
+windows and sentence boundaries on the device, and one fused kernel that trains each kept center over its whole
+window, holding ``W_in[center]`` in registers and pushing it once.
 """
 from __future__ import annotations
 
@@ -25,6 +28,7 @@ from ..errors import FactorIsNotANumberException
 from ..ops import native
 from ..store.replica_cache import ReplicaCache
 from ..store.sharded_table import ShardedTable
+from .w2v_ref import keep_probabilities
 
 ERR_LOGISTIC = 2
 
@@ -34,28 +38,67 @@ def check_noise(noise_counts, vocab: int, noise_power: float) -> np.ndarray:
     non-negative count per word, not all zero, and a finite ``noise_power >= 0``.  Raises ``ValueError``."""
     if not (math.isfinite(float(noise_power)) and float(noise_power) >= 0):
         raise ValueError(f"noise_power must be a finite number >= 0, got {noise_power!r}")
-    c = (noise_counts.detach().cpu().numpy() if torch.is_tensor(noise_counts)
-         else np.asarray(noise_counts)).astype(np.float64).reshape(-1)
+    return _counts(noise_counts, vocab, "noise_counts")
+
+
+def _counts(counts, vocab: int, name: str) -> np.ndarray:
+    c = (counts.detach().cpu().numpy() if torch.is_tensor(counts)
+         else np.asarray(counts)).astype(np.float64).reshape(-1)
     if c.size != int(vocab):
-        raise ValueError(f"noise_counts must hold one count per word of the vocabulary ({vocab}), got {c.size}")
+        raise ValueError(f"{name} must hold one count per word of the vocabulary ({vocab}), got {c.size}")
     if not np.isfinite(c).all():
-        raise ValueError("noise_counts must be finite")
+        raise ValueError(f"{name} must be finite")
     if (c < 0).any():
-        raise ValueError("noise_counts must be >= 0")
+        raise ValueError(f"{name} must be >= 0")
     if not (c > 0).any():
-        raise ValueError("noise_counts must have a positive count for at least one word")
+        raise ValueError(f"{name} must have a positive count for at least one word")
     return c
+
+
+def check_sample(sample) -> float:
+    """Validate the subsampling threshold of :class:`DeviceSkipGram`: a finite number >= 0."""
+    if not (math.isfinite(float(sample)) and float(sample) >= 0):
+        raise ValueError(f"sample must be a finite number >= 0 (0 keeps every word), got {sample!r}")
+    return float(sample)
+
+
+def check_token_call(tokens, window, optimizer: str, sample: float, has_counts: bool) -> None:
+    """The refusals of :meth:`DeviceSkipGram.train_tokens`, each a ``ValueError`` that names the fix."""
+    if optimizer != "sgd":
+        raise ValueError(f"train_tokens trains with plain SGD only, not optimizer={optimizer!r}: build the model "
+                         "with optimizer='sgd', or train (center, context) pairs with step()")
+    if not isinstance(window, (int, np.integer)) or int(window) < 1:
+        raise ValueError(f"window must be an integer >= 1, got {window!r}")
+    if sample > 0 and not has_counts:
+        raise ValueError("sample > 0 needs the corpus counts: pass word_counts (or noise_counts) to DeviceSkipGram, "
+                         "or sample=0 to keep every word")
+    if not torch.is_tensor(tokens) or tokens.dtype not in (torch.int32, torch.int64) or tokens.dim() != 1:
+        raise ValueError("tokens must be a 1-D int32 or int64 tensor of word ids (-1 = sentence boundary); "
+                         "convert with tokens.to(torch.int64)")
+
+
+def expected_records(n_tokens: int, window: int, negative: int) -> int:
+    """Target updates a call of ``n_tokens`` is expected to make with no subsampling and no boundaries: every
+    center has ``window + 1`` contexts on average (a radius uniform on ``1..window``, both sides), each with
+    ``1 + negative`` targets.  Feeds the replica flush policy without reading device counters."""
+    return max(1, int(n_tokens) * (int(window) + 1) * (1 + int(negative)))
 
 
 class DeviceSkipGram:
     def __init__(self, vocab: int, dim: int = 300, learning_rate: float = 0.025, negative: int = 5,
                  group=None, seed: int = 0, device: Optional[int] = None,
                  replica_cache: Optional[bool] = None, sync_every: int = 4, optimizer: str = "sgd",
-                 noise_counts=None, noise_power: float = 0.75):
+                 noise_counts=None, noise_power: float = 0.75, word_counts=None, sample: float = 1e-3):
         """``noise_counts``: ``[vocab]`` word counts.  The negatives are then drawn from ``counts ** noise_power``
         (0.75 is word2vec's choice; words of count 0 are never drawn) by a sampler kernel over an fp64 inverse
-        CDF, instead of uniformly over the vocabulary inside the training kernel.  ``None`` = uniform."""
+        CDF, instead of uniformly over the vocabulary inside the training kernel.  ``None`` = uniform.
+
+        ``word_counts`` (default: ``noise_counts``) are the corpus counts and ``sample`` the threshold of
+        word2vec's frequent-word subsampling in :meth:`train_tokens` (``0`` keeps every word); :meth:`step` does
+        not subsample."""
         noise = check_noise(noise_counts, vocab, noise_power) if noise_counts is not None else None
+        self.sample = check_sample(sample)
+        words = _counts(word_counts, vocab, "word_counts") if word_counts is not None else noise
         if optimizer not in ("sgd", "adagrad"):
             raise ValueError(f"optimizer must be 'sgd' or 'adagrad', got {optimizer!r}")
         self.optimizer = optimizer
@@ -91,6 +134,13 @@ class DeviceSkipGram:
             with torch.cuda.device(self.dev):
                 self._noise_cdf = native.noise_cdf(torch.from_numpy(noise).to(self.dev), self.noise_power)
             self._noise_last = int(np.flatnonzero(noise > 0)[-1])
+        # subsampling: the fp64 keep probability of every word, built once on the host
+        self._keep_p = None
+        if words is not None and self.sample > 0:
+            self._keep_p = torch.from_numpy(keep_probabilities(words, self.sample)).to(self.dev)
+        self._has_counts = words is not None
+        self.token_stats = torch.zeros(4, dtype=torch.int64, device=self.dev)   # tokens, kept, contexts, dropped
+        self._w2v_scratch = None
 
     def step(self, centers: torch.Tensor, contexts: torch.Tensor) -> None:
         if self._ones is None or self._ones.numel() != centers.numel():
@@ -115,6 +165,58 @@ class DeviceSkipGram:
                             reserve_total=(self.rep_in.reserve_total() + self.rep_out.reserve_total())
                             if self.rep_in else 0)
         self.step_no += 1
+
+    def train_tokens(self, tokens: torch.Tensor, window: int = 5, learning_rate: Optional[float] = None) -> None:
+        """Train skip-gram on one micro-batch of text (DESIGN §2.13): ``tokens`` is a 1-D int32 or int64 device
+        tensor of word ids, ``-1`` marking a sentence boundary (any other id outside ``[0, vocab)`` is one too, and
+        is counted as dropped in :attr:`token_stats`).  Frequent words are subsampled with the rule of word2vec.c,
+        each kept center draws a radius on ``1..window`` and trains its contexts within it, never across a
+        boundary or the end of the call, against ``negative`` noise words each.
+
+        Two launches and no host synchronisation; the call uses and advances :attr:`step_no` like :meth:`step`.
+        :attr:`stats` accumulates ``[sum -log sigmoid(+-d), targets trained]`` and :attr:`token_stats` ``[tokens,
+        kept, contexts, dropped]``.  ``learning_rate`` overrides the model's rate for this call."""
+        check_token_call(tokens, window, self.optimizer, self.sample, self._has_counts)
+        if not tokens.is_cuda:
+            tokens = tokens.to(self.dev, non_blocking=True)
+        n = tokens.numel()
+        if self._w2v_scratch is None or self._w2v_scratch[0].numel() < n:
+            self._w2v_scratch = native.w2v_scratch(n, self.dev)
+        tin = self.rep_in.table_c if self.rep_in else self.w_in.table_c
+        tout = self.rep_out.table_c if self.rep_out else self.w_out.table_c
+        if self.rep_in:   # policy + exchange kernels first (side streams), then the training kernels
+            rec = expected_records(n, window, self.negative)
+            self.rep_in.after_step(rec); self.rep_out.after_step(rec)
+        seq, pos, n_comp = native.w2v_subsample(tokens.contiguous(), self.vocab, self._keep_p, seed=self.seed,
+                                                step=self.step_no, token_stats=self.token_stats,
+                                                scratch=self._w2v_scratch)
+        native.w2v_window_fused(seq, pos, n_comp, tin, tout, self.lr if learning_rate is None else learning_rate,
+                                window=int(window), negative=self.negative, vocab=self.vocab, seed=self.seed,
+                                step=self.step_no, cdf=self._noise_cdf, last_nonzero=self._noise_last,
+                                stats=self.stats, token_stats=self.token_stats, nan_flag=self.nan_flag,
+                                reserve_total=(self.rep_in.reserve_total() + self.rep_out.reserve_total())
+                                if self.rep_in else 0)
+        self.step_no += 1
+
+    def fit_tokens(self, tokens: torch.Tensor, epochs: int = 1, batch_tokens: int = 1 << 20, window: int = 5,
+                   min_learning_rate: Optional[float] = None) -> None:
+        """Train on a whole corpus: ``tokens`` (a device tensor, or a host tensor, pinned for asynchronous copies)
+        is cut into calls of ``batch_tokens`` tokens, ``epochs`` times over, through :meth:`train_tokens`.  The
+        rate decays linearly over all tokens of all epochs, as in word2vec.c, from the model's rate to
+        ``min_learning_rate`` (default ``lr * 1e-4``), each call taking the rate at its first token."""
+        if int(epochs) < 1 or int(batch_tokens) < 1:
+            raise ValueError("epochs and batch_tokens must be >= 1")
+        check_token_call(tokens, window, self.optimizer, self.sample, self._has_counts)
+        floor = self.lr * 1e-4 if min_learning_rate is None else float(min_learning_rate)
+        n = tokens.numel()
+        total = max(1, n * int(epochs))
+        done = 0
+        for _ in range(int(epochs)):
+            for lo in range(0, n, int(batch_tokens)):
+                batch = tokens[lo:lo + int(batch_tokens)]
+                lr = max(floor, self.lr * (1.0 - done / total))
+                self.train_tokens(batch, window=window, learning_rate=lr)
+                done += batch.numel()
 
     def flush(self) -> None:
         if self.rep_in:

@@ -782,6 +782,136 @@ def neg_sample_noise(users: torch.Tensor, items: Optional[torch.Tensor], ratings
     return out
 
 
+class W2vArgsC(C.Structure):
+    """Mirror of ``struct W2vArgs`` (csrc/fps_w2v_window.cu)."""
+
+    _fields_ = [
+        ("tokens", C.c_void_p), ("n_tokens", C.c_longlong), ("vocab", C.c_longlong), ("keep_p", C.c_void_p),
+        ("seed", C.c_ulonglong), ("step", C.c_ulonglong),
+        ("seq", C.c_void_p), ("pos", C.c_void_p), ("n_comp", C.c_void_p), ("cta_cnt", C.c_void_p),
+        ("cta_cap", C.c_int), ("stride", C.c_int), ("token_stats", C.c_void_p),
+        ("w_in", ShardTableC), ("w_out", ShardTableC),
+        ("window", C.c_int), ("negative", C.c_int), ("max_tries", C.c_int), ("lr", C.c_float),
+        ("cdf", C.c_void_p), ("last_nonzero", C.c_longlong), ("stats", C.c_void_p), ("nan_flag", C.c_void_p),
+        ("reserve_total", C.c_int), ("pad_", C.c_int),
+    ]
+
+
+def w2v_scratch(n_tokens: int, device) -> tuple:
+    """Device scratch of :func:`w2v_subsample` for calls of up to ``n_tokens`` tokens: ``(seq, pos, n_comp,
+    cta_cnt)`` int32 ``[n_tokens]``, ``[n_tokens]``, ``[1]`` and ``[8 * SMs]``.  Reusable from call to call."""
+    n = max(int(n_tokens), 1)
+    dev = torch.device(device)
+    return (torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
+            torch.zeros(1, dtype=torch.int32, device=dev),
+            torch.empty(sm_count(dev.index) * 8, dtype=torch.int32, device=dev))
+
+
+def w2v_subsample(tokens: torch.Tensor, vocab: int, keep_p: Optional[torch.Tensor] = None, *, seed: int = 0,
+                  step: int = 0, token_stats: Optional[torch.Tensor] = None, scratch: Optional[tuple] = None) -> tuple:
+    """Frequent-word subsampling and compaction of one token call (csrc/fps_w2v_window.cu, DESIGN §2.13), in one
+    cooperative launch with no host synchronisation.
+
+    ``tokens``: 1-D int32 or int64 CUDA tensor; ``-1`` marks a sentence boundary, and so does any other id outside
+    ``[0, vocab)`` (counted as dropped).  Word ``w`` at call position ``i`` is kept iff the 53-bit Philox uniform
+    keyed ``(i, 0, 0, step; seed)`` is ``< keep_p[w]`` (float64 ``[vocab]``; ``None`` keeps every word).  The kept
+    words and every boundary, in order, form the compacted sequence.
+
+    Returns ``(seq, pos, n_comp)``: int32 compacted sequence (``-1`` = boundary), the call position of each
+    entry, and an int32 ``[1]`` device tensor holding the compacted length; only the first ``n_comp`` entries are
+    written.  ``scratch`` (:func:`w2v_scratch`, large enough) is used instead of fresh buffers.  ``token_stats``
+    (int64 ``[4]``) accumulates the tokens, the kept words and, at index 3, the dropped ids."""
+    _req(tokens, "tokens")
+    idb = _id_bytes(tokens)
+    n = tokens.numel()
+    if scratch is None:
+        scratch = w2v_scratch(n, tokens.device)
+    seq, pos, n_comp, cta_cnt = scratch
+    for t, name in ((seq, "seq"), (pos, "pos"), (n_comp, "n_comp"), (cta_cnt, "cta_cnt")):
+        _req(t, name, torch.int32)
+    if seq.numel() < n or pos.numel() < n:
+        raise ValueError(f"scratch holds {seq.numel()} entries, the call has {n} tokens")
+    if n >= 2**31 - 1:
+        raise ValueError("a token call must hold fewer than 2**31 - 1 tokens")
+    a = W2vArgsC()
+    a.tokens, a.n_tokens, a.vocab = tokens.data_ptr(), n, int(vocab)
+    if keep_p is not None:
+        _req(keep_p, "keep_p", torch.float64)
+        if keep_p.numel() != int(vocab):
+            raise ValueError("keep_p must hold one probability per word")
+        a.keep_p = keep_p.data_ptr()
+    a.seed = seed & (2**64 - 1); a.step = int(step)
+    a.seq, a.pos, a.n_comp, a.cta_cnt = seq.data_ptr(), pos.data_ptr(), n_comp.data_ptr(), cta_cnt.data_ptr()
+    a.cta_cap = cta_cnt.numel()
+    if token_stats is not None:
+        _req(token_stats, "token_stats", torch.int64)
+        a.token_stats = token_stats.data_ptr()
+    if n == 0:
+        n_comp.zero_()
+        return seq, pos, n_comp
+    _check(lib().fps_w2v_subsample(C.byref(a), idb, sm_count(tokens.device.index), _stream()), "w2v_subsample")
+    _bump()
+    return seq, pos, n_comp
+
+
+def w2v_window_fused(seq: torch.Tensor, pos: torch.Tensor, n_comp: torch.Tensor, w_in: ShardTableC,
+                     w_out: ShardTableC, lr: float, *, window: int = 5, negative: int = 5, vocab: int,
+                     seed: int = 0, step: int = 0, cdf: Optional[torch.Tensor] = None, last_nonzero: int = 0,
+                     max_tries: int = 32, stats: Optional[torch.Tensor] = None,
+                     token_stats: Optional[torch.Tensor] = None, nan_flag: Optional[torch.Tensor] = None,
+                     reserve_total: int = 0) -> None:
+    """Fused center-window skip-gram negative-sampling step (csrc/fps_w2v_window.cu, DESIGN §2.13) over the
+    compacted sequence of :func:`w2v_subsample`; one lane-group per kept center, the grid sized without reading
+    ``n_comp`` on the host.
+
+    The center at call position ``i`` draws a radius ``r = 1 + h mod window`` (``h`` keyed ``(i, 1, 0, step)``);
+    its contexts are the entries up to ``r`` positions to either side, stopping at a boundary, in increasing
+    position.  Each context ``q`` trains the context word (label 1), then ``negative`` noise words (label 0),
+    uniform over ``[0, vocab)`` or from ``cdf`` (:func:`noise_cdf`, ``last_nonzero`` its last word of positive
+    weight), keyed ``(i, 2 | slot << 8, j | try << 8, step)``; a draw equal to the context word is redrawn up to
+    ``max_tries`` times, then voided.  With ``u = W_in[center]`` as pulled and ``D = 0``, per target
+    ``d = (u + D) . v``, ``g = lr (label - sigmoid(d))``; ``g (u + D)`` is pushed to ``W_out[t]`` at once, ``g v``
+    summed into the context's ``e``, and ``D += e`` after the context.  ``D`` is pushed to ``W_in[center]`` once.
+
+    ``w_in`` / ``w_out``: :class:`ShardTableC` of the same stride, at most 512 floats.  ``stats`` (float32 ``[2]``)
+    accumulates ``sum -log sigmoid(+-d)`` and the targets trained, ``token_stats`` (int64 ``[4]``) the contexts at
+    index 2, ``nan_flag`` is set by a non-finite ``d``.  ``reserve_total``: CTA slots left free for the replica
+    exchange running next to it."""
+    for t, name in ((seq, "seq"), (pos, "pos"), (n_comp, "n_comp")):
+        _req(t, name, torch.int32)
+    if int(w_in.stride) != int(w_out.stride):
+        raise ValueError("w_in and w_out must have the same stride")
+    if not 1 <= int(window) < 2**23:
+        raise ValueError(f"window must be in [1, 2**23), got {window!r}")
+    if not 0 <= int(negative) <= 255:
+        raise ValueError(f"negative must be in [0, 255], got {negative!r}")
+    if not 1 <= int(max_tries) < 2**23:
+        raise ValueError(f"max_tries must be in [1, 2**23), got {max_tries!r}")
+    a = W2vArgsC()
+    a.n_tokens, a.vocab = seq.numel(), int(vocab)
+    a.seq, a.pos, a.n_comp = seq.data_ptr(), pos.data_ptr(), n_comp.data_ptr()
+    a.w_in, a.w_out, a.stride = w_in, w_out, int(w_in.stride)
+    a.window, a.negative, a.max_tries, a.lr = int(window), int(negative), int(max_tries), float(lr)
+    a.seed = seed & (2**64 - 1); a.step = int(step)
+    if cdf is not None:
+        _req(cdf, "cdf", torch.float64)
+        if cdf.numel() != int(vocab) or not 0 <= int(last_nonzero) < cdf.numel():
+            raise ValueError("cdf must hold one prefix per word and last_nonzero must index it")
+        a.cdf, a.last_nonzero = cdf.data_ptr(), int(last_nonzero)
+    if stats is not None:
+        _req(stats, "stats", torch.float32)
+        a.stats = stats.data_ptr()
+    if token_stats is not None:
+        _req(token_stats, "token_stats", torch.int64)
+        a.token_stats = token_stats.data_ptr()
+    if nan_flag is not None:
+        _req(nan_flag, "nan_flag", torch.int32)
+        a.nan_flag = nan_flag.data_ptr()
+    a.reserve_total = int(reserve_total)
+    _check(lib().fps_w2v_window_fused(C.byref(a), sm_count(seq.device.index), _stream()), "w2v_window_fused")
+    _bump()
+
+
 class BucketArgsC(C.Structure):
     """Mirror of ``struct BucketArgs`` (csrc/fps_bucket.cu)."""
 

@@ -66,3 +66,29 @@ def lowrank_implicit(num_users: int, num_items: int, per_user: int, held_out: in
     tr_u, tr_i = torch.cat(tr_u), torch.cat(tr_i)
     perm = torch.randperm(tr_u.numel(), generator=g)
     return tr_u[perm], tr_i[perm], torch.cat(te_u), torch.cat(te_i)
+
+
+def topic_corpus(vocab: int, topics: int, sentence_len: int, sentences: int, seed: int = 0,
+                 zipf: float = 1.0) -> torch.Tensor:
+    """A seeded token stream with known neighbours for word2vec: word ``w`` belongs to topic ``w % topics``, each
+    sentence draws one topic uniformly and ``sentence_len`` words of it, the word of rank ``w // topics`` in its
+    topic with weight ``1 / (rank + 1) ** zipf``.  So low ids are frequent (a Zipf-like corpus that subsampling
+    acts on) and two words are true neighbours iff they share a topic.
+
+    Returns a 1-D int64 CPU tensor: the sentences, each followed by ``-1`` (a sentence boundary)."""
+    if not 1 <= topics <= vocab or sentence_len < 1 or sentences < 1:
+        raise ValueError("need 1 <= topics <= vocab, sentence_len >= 1 and sentences >= 1")
+    g = torch.Generator().manual_seed(int(seed))
+    per = -(-vocab // topics)                             # ranks in the largest topic
+    rank = torch.arange(per, dtype=torch.float64)
+    topic = torch.randint(0, topics, (sentences,), generator=g)
+    size = (vocab - 1 - torch.arange(topics)) // topics + 1   # words of each topic
+    out = torch.full((sentences, sentence_len + 1), -1, dtype=torch.int64)
+    for k in range(topics):
+        rows = torch.nonzero(topic == k).flatten()
+        if rows.numel() == 0:
+            continue
+        w = (rank[: int(size[k])] + 1.0) ** -float(zipf)
+        r = torch.multinomial(w, rows.numel() * sentence_len, replacement=True, generator=g)
+        out[rows, :sentence_len] = (r * topics + k).view(rows.numel(), sentence_len)
+    return out.reshape(-1)
