@@ -118,23 +118,27 @@ def negative(i: int, slot: int, j: int, ctx: int, vocab: int, step: int, seed: i
 
 def center_targets(i: int, contexts_words, negative_count: int, vocab: int, step: int, seed: int,
                    philox: Callable, **noise) -> List[List[Tuple[int, float]]]:
-    """``[[(word, label), ...] per context]``: the context word with label 1, then its ``negative_count`` noise
-    words with label 0 (void draws left out)."""
+    """``[[(word, label), ...] per context]``: the context's target slots ``0 .. negative_count``, the context word
+    with label 1, then its noise words with label 0.  A void draw keeps its slot as ``(-1, 0.0)``."""
     out = []
     for slot, ctx in enumerate(contexts_words):
         tg = [(int(ctx), 1.0)]
         for j in range(negative_count):
-            w = negative(i, slot, j, int(ctx), vocab, step, seed, philox, **noise)
-            if w >= 0:
-                tg.append((w, 0.0))
+            tg.append((negative(i, slot, j, int(ctx), vocab, step, seed, philox, **noise), 0.0))
         out.append(tg)
     return out
 
 
+def target_block(width: int) -> int:
+    """Target slots the kernel pulls per block for rows of ``width`` floats: 8, or 6 over 384 floats."""
+    return 6 if int(width) > 384 else 8
+
+
 def center_update(u: np.ndarray, w_out: np.ndarray, targets, lr: float, block: int = 8):
     """The update of one center (DESIGN §2.13) applied in place to ``w_out`` (rows indexed by word).  ``u`` is the
-    center's row as pulled; returns ``(D, loss)``, the delta to add to it and ``sum -log sigmoid(+-d)``.  Targets
-    are read in blocks of ``block`` rows: a row repeated inside a block is read as it was before the block."""
+    center's row as pulled; returns ``(D, loss)``, the delta to add to it and ``sum -log sigmoid(+-d)``.  Each
+    context's targets (:func:`center_targets`) are read in blocks of ``block`` slots, a void slot (word ``-1``)
+    included and then skipped: a row repeated inside a block is read as it was before the block."""
     dt = u.dtype
     D = np.zeros_like(u)
     loss = 0.0
@@ -142,7 +146,7 @@ def center_update(u: np.ndarray, w_out: np.ndarray, targets, lr: float, block: i
         w = u + D
         e = np.zeros_like(u)
         for b0 in range(0, len(tg), block):
-            blk = tg[b0:b0 + block]
+            blk = [(t, label) for t, label in tg[b0:b0 + block] if t >= 0]
             vs = [w_out[t].copy() for t, _ in blk]
             for (t, label), v in zip(blk, vs):
                 d = dt.type(np.dot(w, v))
@@ -158,17 +162,19 @@ def train_call(w_in: np.ndarray, w_out: np.ndarray, tokens, *, lr: float, window
                step: int, seed: int, philox: Callable, p: Optional[np.ndarray] = None, cdf=None,
                last_nonzero: int = 0, max_tries: int = 32) -> dict:
     """One :meth:`DeviceSkipGram.train_tokens` call applied sequentially, center by center in compacted order, to
-    the tables in place.  Returns the counters ``tokens, kept, contexts, dropped`` and ``loss, targets``."""
+    the tables in place, in target blocks of :func:`target_block` of the row width.  Returns the counters
+    ``tokens, kept, contexts, dropped`` and ``loss, targets`` (void draws are not targets)."""
     vocab = w_in.shape[0]
+    block = target_block(w_in.shape[1])
     seq, pos, kept, dropped = compact(tokens, vocab, p, step, seed, philox)
     loss, n_tgt, n_ctx = 0.0, 0, 0
     for e, ctx in windows(seq, pos, window, step, seed, philox):
         tg = center_targets(int(pos[e]), seq[ctx], negative_count, vocab, step, seed, philox, cdf=cdf,
                             last_nonzero=last_nonzero, max_tries=max_tries)
-        D, l = center_update(w_in[seq[e]].copy(), w_out, tg, lr)
+        D, l = center_update(w_in[seq[e]].copy(), w_out, tg, lr, block)
         w_in[seq[e]] += D
         loss += l
-        n_tgt += sum(len(t) for t in tg)
+        n_tgt += sum(t >= 0 for c in tg for t, _ in c)
         n_ctx += len(ctx)
     return dict(tokens=len(np.asarray(tokens)), kept=kept, contexts=n_ctx, dropped=dropped, loss=loss,
                 targets=n_tgt)

@@ -61,7 +61,7 @@ def _collision_free_corpus(vocab, n_sent, neg, window, seed, cdf=None, last=0):
         rep = _replay(tok, vocab, window, neg, 0, seed, cdf, last)
         readers = {}
         for c, tg in rep:
-            for w in {t for ctx in tg for t, _ in ctx}:
+            for w in {t for ctx in tg for t, _ in ctx if t >= 0}:
                 readers.setdefault(w, set()).add(c)
         shared = {w for w, cs in readers.items() if len(cs) > 1}
         bad = {c for c, tg in rep if any(t in shared for ctx in tg for t, _ in ctx)}
@@ -96,7 +96,7 @@ def test_fused_kernel_matches_fp32_oracle(dev, dim, noise):
     W_in, W_out = Win.copy(), Wout.copy()
     loss = 0.0
     for c, tg in rep:
-        D, lsum = R.center_update(Win[c].copy(), W_out, tg, lr, block=6 if dim > 384 else 8)
+        D, lsum = R.center_update(Win[c].copy(), W_out, tg, lr, block=R.target_block(dim))
         W_in[c] += D
         loss += lsum
     m.train_tokens(torch.from_numpy(tok).to(dev), window=window)
@@ -106,7 +106,7 @@ def test_fused_kernel_matches_fp32_oracle(dev, dim, noise):
     np.testing.assert_allclose(got_out, W_out, rtol=1e-5, atol=1e-7)
     untouched = np.setdiff1d(np.arange(vocab), np.array(reads))
     assert np.array_equal(got_in[untouched], Win[untouched]) and np.array_equal(got_out[untouched], Wout[untouched])
-    n_tgt = sum(len(ctx) for _, tg in rep for ctx in tg)
+    n_tgt = sum(t >= 0 for _, tg in rep for ctx in tg for t, _ in ctx)
     st, ts = m.stats.cpu(), m.token_stats.cpu()
     assert st[1].item() == n_tgt and abs(st[0].item() - loss) < 1e-4 * loss
     assert ts.tolist() == [len(tok), int((tok >= 0).sum()), sum(len(tg) for _, tg in rep), 0]

@@ -115,6 +115,74 @@ def test_later_contexts_read_the_earlier_updates():
     np.testing.assert_allclose(W2[0], v1 + g2 * w2, rtol=1e-5)
 
 
+def _one_context_in_blocks(u, W, blocks, lr):
+    """One context trained block by block: all rows of a block pulled, then each target's update."""
+    e = np.zeros_like(u)
+    for blk in blocks:
+        vs = [W[t].copy() for t, _ in blk]
+        for (t, label), v in zip(blk, vs):
+            g = lr * (label - 1.0 / (1.0 + np.exp(-np.dot(u, v))))
+            e += g * v
+            W[t] += g * u
+    return e
+
+
+def test_void_draw_keeps_its_target_slot():
+    """Blocks are made of target slots 0 .. negative: a voided draw keeps its slot, so the next block starts at
+    slot 8 whether or not a draw before it was voided.  Sentence ``0 1`` of a 3-word vocabulary, one try per draw:
+    the center 0 trains [1, 2, 2] and then [2, 2, 0, 0], not [1, 2, 2, 2, 2, 0, 0] in one block."""
+    tg = R.center_targets(0, [1], 12, 3, step=0, seed=4, philox=PH, max_tries=1)
+    assert tg == [[(1, 1.0)] + [(-1, 0.0)] * 5 + [(2, 0.0)] * 4 + [(-1, 0.0)] + [(0, 0.0)] * 2]
+    rng = np.random.default_rng(3)
+    u, W0 = rng.uniform(-0.5, 0.5, 8), rng.uniform(-0.5, 0.5, (3, 8))
+    W = W0.copy()
+    D, _ = R.center_update(u, W, tg, 0.1, block=8)
+    by_slot = W0.copy()
+    e = _one_context_in_blocks(u, by_slot, [[(1, 1.0), (2, 0.0), (2, 0.0)],
+                                            [(2, 0.0), (2, 0.0), (0, 0.0), (0, 0.0)]], 0.1)
+    np.testing.assert_allclose(W, by_slot, rtol=1e-13, atol=1e-15)
+    np.testing.assert_allclose(D, e, rtol=1e-13, atol=1e-15)
+    compacted = W0.copy()
+    e_c = _one_context_in_blocks(u, compacted, [[(1, 1.0)] + [(2, 0.0)] * 4 + [(0, 0.0)] * 2], 0.1)
+    assert np.abs(compacted - W).max() > 1e-3 and np.abs(e_c - D).max() > 1e-3
+    # counters leave the voids out
+    w_in, w_out = rng.uniform(-0.5, 0.5, (3, 8)), rng.uniform(-0.5, 0.5, (3, 8))
+    st = R.train_call(w_in, w_out, np.array([0, 1]), lr=0.1, window=1, negative_count=12, step=0, seed=4,
+                      philox=PH, max_tries=1)
+    tg1 = R.center_targets(1, [0], 12, 3, step=0, seed=4, philox=PH, max_tries=1)
+    assert st["contexts"] == 2 and st["targets"] == 7 + sum(t >= 0 for t, _ in tg1[0])
+
+
+def _replay_in_blocks(w_in, w_out, tokens, block, *, lr, neg, seed):
+    seq, pos, _, _ = R.compact(tokens, len(w_in), None, 0, seed, PH)
+    for e, ctx in R.windows(seq, pos, 1, 0, seed, PH):
+        tg = R.center_targets(int(pos[e]), seq[ctx], neg, len(w_in), 0, seed, PH)
+        D, _ = R.center_update(w_in[seq[e]].copy(), w_out, tg, lr, block)
+        w_in[seq[e]] += D
+
+
+@pytest.mark.parametrize("width,block", [(388, 6), (384, 8)])
+def test_train_call_takes_the_target_block_from_the_row_width(width, block):
+    """Rows over 384 floats are pulled 6 target slots at a time.  With seed 0, word 0 sits in slots 1, 2 and 6 of
+    the center 0's targets: a block of 6 reads it in slot 6 with the earlier pushes applied, a block of 8 as it
+    was before the block."""
+    vocab, neg, lr, seed = 4, 7, 0.1, 0
+    tokens = np.array([0, 1])
+    assert [t for t, _ in R.center_targets(0, [1], neg, vocab, 0, seed, PH)[0]] == [1, 0, 0, 2, 3, 2, 0, 2]
+    assert R.target_block(width) == block
+    rng = np.random.default_rng(1)
+    w_in, w_out = rng.uniform(-0.5, 0.5, (vocab, width)), rng.uniform(-0.5, 0.5, (vocab, width))
+    got_in, got_out = w_in.copy(), w_out.copy()
+    R.train_call(got_in, got_out, tokens, lr=lr, window=1, negative_count=neg, step=0, seed=seed, philox=PH)
+    res = {}
+    for b in (6, 8):
+        a, o = w_in.copy(), w_out.copy()
+        _replay_in_blocks(a, o, tokens, b, lr=lr, neg=neg, seed=seed)
+        res[b] = a, o
+    assert np.array_equal(got_in, res[block][0]) and np.array_equal(got_out, res[block][1])
+    assert np.abs(res[6][1] - res[8][1]).max() > 1e-3 and np.abs(res[6][0] - res[8][0]).max() > 1e-3
+
+
 def test_topic_corpus_is_seeded_and_topical():
     a, b = topic_corpus(100, 5, 8, 50, seed=3), topic_corpus(100, 5, 8, 50, seed=3)
     assert torch.equal(a, b) and a.dtype == torch.int64 and a.numel() == 50 * 9
