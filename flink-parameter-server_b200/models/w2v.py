@@ -13,7 +13,9 @@ accumulator per row of each table on that row's shard.  ``noise_counts`` draws t
 noise ``counts ** noise_power`` (Mikolov et al. 2013) instead (DESIGN §2.11).
 ``train_tokens`` / ``fit_tokens`` train from a token stream (DESIGN §2.13): frequent-word subsampling, dynamic
 windows and sentence boundaries on the device, and one fused kernel that trains each kept center over its whole
-window, holding ``W_in[center]`` in registers and pushing it once.
+window, holding ``W_in[center]`` in registers and pushing it once.  ``cbow=True`` trains CBOW on the same windows
+(DESIGN §2.14): one fused kernel averages the context rows, trains the center word against the noise words and
+pushes the error to every context row.
 """
 from __future__ import annotations
 
@@ -62,8 +64,11 @@ def check_sample(sample) -> float:
     return float(sample)
 
 
-def check_token_call(tokens, window, optimizer: str, sample: float, has_counts: bool) -> None:
+def check_token_call(tokens, window, optimizer: str, sample: float, has_counts: bool, cbow=False) -> None:
     """The refusals of :meth:`DeviceSkipGram.train_tokens`, each a ``ValueError`` that names the fix."""
+    if not isinstance(cbow, bool):
+        raise ValueError(f"cbow must be True (CBOW) or False (skip-gram), got {cbow!r}: pass a bool, "
+                         "e.g. cbow=bool(flag)")
     if optimizer != "sgd":
         raise ValueError(f"train_tokens trains with plain SGD only, not optimizer={optimizer!r}: build the model "
                          "with optimizer='sgd', or train (center, context) pairs with step()")
@@ -77,10 +82,13 @@ def check_token_call(tokens, window, optimizer: str, sample: float, has_counts: 
                          "convert with tokens.to(torch.int64)")
 
 
-def expected_records(n_tokens: int, window: int, negative: int) -> int:
-    """Target updates a call of ``n_tokens`` is expected to make with no subsampling and no boundaries: every
+def expected_records(n_tokens: int, window: int, negative: int, cbow: bool = False) -> int:
+    """Row pushes a call of ``n_tokens`` is expected to make with no subsampling and no boundaries: every
     center has ``window + 1`` contexts on average (a radius uniform on ``1..window``, both sides), each with
-    ``1 + negative`` targets.  Feeds the replica flush policy without reading device counters."""
+    ``1 + negative`` targets in skip-gram.  A CBOW center pushes its ``1 + negative`` targets once and then every
+    context row.  Feeds the replica flush policy without reading device counters."""
+    if cbow:
+        return max(1, int(n_tokens) * ((1 + int(negative)) + (int(window) + 1)))
     return max(1, int(n_tokens) * (int(window) + 1) * (1 + int(negative)))
 
 
@@ -166,17 +174,23 @@ class DeviceSkipGram:
                             if self.rep_in else 0)
         self.step_no += 1
 
-    def train_tokens(self, tokens: torch.Tensor, window: int = 5, learning_rate: Optional[float] = None) -> None:
+    def train_tokens(self, tokens: torch.Tensor, window: int = 5, learning_rate: Optional[float] = None,
+                     cbow: bool = False) -> None:
         """Train skip-gram on one micro-batch of text (DESIGN §2.13): ``tokens`` is a 1-D int32 or int64 device
         tensor of word ids, ``-1`` marking a sentence boundary (any other id outside ``[0, vocab)`` is one too, and
         is counted as dropped in :attr:`token_stats`).  Frequent words are subsampled with the rule of word2vec.c,
         each kept center draws a radius on ``1..window`` and trains its contexts within it, never across a
         boundary or the end of the call, against ``negative`` noise words each.
 
+        ``cbow=True`` trains CBOW on the same windows instead (DESIGN §2.14): the mean of a center's context rows
+        predicts the center word against ``negative`` noise words, and the error is added, unscaled, to every
+        context row, as word2vec.c does.  word2vec.c's default rate for CBOW is 0.05 (0.025 for skip-gram); the
+        model's rate is used as given.
+
         Two launches and no host synchronisation; the call uses and advances :attr:`step_no` like :meth:`step`.
         :attr:`stats` accumulates ``[sum -log sigmoid(+-d), targets trained]`` and :attr:`token_stats` ``[tokens,
         kept, contexts, dropped]``.  ``learning_rate`` overrides the model's rate for this call."""
-        check_token_call(tokens, window, self.optimizer, self.sample, self._has_counts)
+        check_token_call(tokens, window, self.optimizer, self.sample, self._has_counts, cbow)
         if not tokens.is_cuda:
             tokens = tokens.to(self.dev, non_blocking=True)
         n = tokens.numel()
@@ -185,7 +199,7 @@ class DeviceSkipGram:
         tin = self.rep_in.table_c if self.rep_in else self.w_in.table_c
         tout = self.rep_out.table_c if self.rep_out else self.w_out.table_c
         if self.rep_in:   # policy + exchange kernels first (side streams), then the training kernels
-            rec = expected_records(n, window, self.negative)
+            rec = expected_records(n, window, self.negative, cbow)
             self.rep_in.after_step(rec); self.rep_out.after_step(rec)
         seq, pos, n_comp = native.w2v_subsample(tokens.contiguous(), self.vocab, self._keep_p, seed=self.seed,
                                                 step=self.step_no, token_stats=self.token_stats,
@@ -195,18 +209,19 @@ class DeviceSkipGram:
                                 step=self.step_no, cdf=self._noise_cdf, last_nonzero=self._noise_last,
                                 stats=self.stats, token_stats=self.token_stats, nan_flag=self.nan_flag,
                                 reserve_total=(self.rep_in.reserve_total() + self.rep_out.reserve_total())
-                                if self.rep_in else 0)
+                                if self.rep_in else 0, cbow=cbow)
         self.step_no += 1
 
     def fit_tokens(self, tokens: torch.Tensor, epochs: int = 1, batch_tokens: int = 1 << 20, window: int = 5,
-                   min_learning_rate: Optional[float] = None) -> None:
+                   min_learning_rate: Optional[float] = None, cbow: bool = False) -> None:
         """Train on a whole corpus: ``tokens`` (a device tensor, or a host tensor, pinned for asynchronous copies)
         is cut into calls of ``batch_tokens`` tokens, ``epochs`` times over, through :meth:`train_tokens`.  The
         rate decays linearly over all tokens of all epochs, as in word2vec.c, from the model's rate to
-        ``min_learning_rate`` (default ``lr * 1e-4``), each call taking the rate at its first token."""
+        ``min_learning_rate`` (default ``lr * 1e-4``), each call taking the rate at its first token.  ``cbow``
+        selects CBOW as in :meth:`train_tokens`."""
         if int(epochs) < 1 or int(batch_tokens) < 1:
             raise ValueError("epochs and batch_tokens must be >= 1")
-        check_token_call(tokens, window, self.optimizer, self.sample, self._has_counts)
+        check_token_call(tokens, window, self.optimizer, self.sample, self._has_counts, cbow)
         floor = self.lr * 1e-4 if min_learning_rate is None else float(min_learning_rate)
         n = tokens.numel()
         total = max(1, n * int(epochs))
@@ -215,7 +230,7 @@ class DeviceSkipGram:
             for lo in range(0, n, int(batch_tokens)):
                 batch = tokens[lo:lo + int(batch_tokens)]
                 lr = max(floor, self.lr * (1.0 - done / total))
-                self.train_tokens(batch, window=window, learning_rate=lr)
+                self.train_tokens(batch, window=window, learning_rate=lr, cbow=cbow)
                 done += batch.numel()
 
     def flush(self) -> None:

@@ -1,5 +1,6 @@
 """NumPy reference of :meth:`DeviceSkipGram.train_tokens` (DESIGN §2.13): the keep probabilities, the Philox draws
-of subsampling, dynamic windows and negatives, the compaction, and the center-window SGNS update.
+of subsampling, dynamic windows and negatives, the compaction, the center-window SGNS update, and the CBOW update of
+``train_tokens(cbow=True)`` (DESIGN §2.14).
 
 Every draw is a Philox4x32-10 value with counter ``(c0, c1, c2, c3)`` and key ``(seed lo, seed hi)``, where ``i`` is
 the token's position in the call.  The functions take the generator as ``philox(c0, c1, c2, c3, k0, k1) -> (x, y,
@@ -158,19 +159,64 @@ def center_update(u: np.ndarray, w_out: np.ndarray, targets, lr: float, block: i
     return D, loss
 
 
+def cbow_update(w_in: np.ndarray, w_out: np.ndarray, context_words, targets, lr: float, block: int = 8):
+    """The CBOW update of one center (DESIGN §2.14) applied in place to both tables.  ``h`` is the mean of the
+    ``context_words`` rows of ``w_in`` as pulled, summed in the order given (a repeated word counts each time);
+    ``targets`` is the center's one slot list (``[(center, 1.0), noise ...]``), trained on ``h`` by
+    :func:`center_update`, which returns the error ``e``.  ``e`` is then added, unscaled, to the row of every
+    context word, once per occurrence.  Returns ``(e, loss)``; with no context words nothing changes."""
+    if len(context_words) == 0:
+        return np.zeros(w_in.shape[1], dtype=w_in.dtype), 0.0
+    rows = [w_in[c].copy() for c in context_words]
+    h = np.zeros_like(rows[0])
+    for r in rows:
+        h += r
+    h /= w_in.dtype.type(len(rows))
+    e, loss = center_update(h, w_out, [targets], lr, block)
+    for c in context_words:
+        w_in[c] += e
+    return e, loss
+
+
+def cbow_centers(seq, pos, window: int, negative_count: int, vocab: int, step: int, seed: int, philox: Callable,
+                 **noise) -> List[Tuple[List[int], List[Tuple[int, float]]]]:
+    """``[(context words, targets)]`` of every CBOW center with at least one context, in compacted order: the
+    context words in increasing position, and the targets of :func:`center_targets` for the center word alone, so
+    the noise words are those of context slot 0, rejected against the center word."""
+    seq = np.asarray(seq)
+    out = []
+    for e, ctx in windows(seq, pos, window, step, seed, philox):
+        if ctx:
+            tg = center_targets(int(pos[e]), [seq[e]], negative_count, vocab, step, seed, philox, **noise)[0]
+            out.append(([int(c) for c in seq[ctx]], tg))
+    return out
+
+
 def train_call(w_in: np.ndarray, w_out: np.ndarray, tokens, *, lr: float, window: int, negative_count: int,
                step: int, seed: int, philox: Callable, p: Optional[np.ndarray] = None, cdf=None,
-               last_nonzero: int = 0, max_tries: int = 32) -> dict:
+               last_nonzero: int = 0, max_tries: int = 32, cbow: bool = False, order=None) -> dict:
     """One :meth:`DeviceSkipGram.train_tokens` call applied sequentially, center by center in compacted order, to
-    the tables in place, in target blocks of :func:`target_block` of the row width.  Returns the counters
-    ``tokens, kept, contexts, dropped`` and ``loss, targets`` (void draws are not targets)."""
+    the tables in place, in target blocks of :func:`target_block` of the row width.  ``cbow=True`` replays CBOW
+    (:func:`cbow_update`; the negatives are those of context slot 0, rejected against the center word).  ``order``
+    ``"reverse"`` applies the centers last to first.  Returns the counters ``tokens, kept, contexts, dropped`` and
+    ``loss, targets`` (void draws are not targets; a CBOW center with no context trains and counts nothing)."""
     vocab = w_in.shape[0]
     block = target_block(w_in.shape[1])
     seq, pos, kept, dropped = compact(tokens, vocab, p, step, seed, philox)
     loss, n_tgt, n_ctx = 0.0, 0, 0
-    for e, ctx in windows(seq, pos, window, step, seed, philox):
-        tg = center_targets(int(pos[e]), seq[ctx], negative_count, vocab, step, seed, philox, cdf=cdf,
-                            last_nonzero=last_nonzero, max_tries=max_tries)
+    noise = dict(cdf=cdf, last_nonzero=last_nonzero, max_tries=max_tries)
+    if cbow:
+        plan = cbow_centers(seq, pos, window, negative_count, vocab, step, seed, philox, **noise)
+        for ctx, tg in (plan[::-1] if order == "reverse" else plan):
+            _, l = cbow_update(w_in, w_out, ctx, tg, lr, block)
+            loss += l
+            n_tgt += sum(t >= 0 for t, _ in tg)
+            n_ctx += len(ctx)
+        return dict(tokens=len(np.asarray(tokens)), kept=kept, contexts=n_ctx, dropped=dropped, loss=loss,
+                    targets=n_tgt)
+    wins = windows(seq, pos, window, step, seed, philox)
+    for e, ctx in (wins[::-1] if order == "reverse" else wins):
+        tg = center_targets(int(pos[e]), seq[ctx], negative_count, vocab, step, seed, philox, **noise)
         D, l = center_update(w_in[seq[e]].copy(), w_out, tg, lr, block)
         w_in[seq[e]] += D
         loss += l

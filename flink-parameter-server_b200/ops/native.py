@@ -859,10 +859,10 @@ def w2v_window_fused(seq: torch.Tensor, pos: torch.Tensor, n_comp: torch.Tensor,
                      seed: int = 0, step: int = 0, cdf: Optional[torch.Tensor] = None, last_nonzero: int = 0,
                      max_tries: int = 32, stats: Optional[torch.Tensor] = None,
                      token_stats: Optional[torch.Tensor] = None, nan_flag: Optional[torch.Tensor] = None,
-                     reserve_total: int = 0) -> None:
+                     reserve_total: int = 0, cbow: bool = False) -> None:
     """Fused center-window skip-gram negative-sampling step (csrc/fps_w2v_window.cu, DESIGN §2.13) over the
     compacted sequence of :func:`w2v_subsample`; one lane-group per kept center, the grid sized without reading
-    ``n_comp`` on the host.
+    ``n_comp`` on the host.  ``cbow=True`` runs the CBOW kernel instead (DESIGN §2.14), described below.
 
     The center at call position ``i`` draws a radius ``r = 1 + h mod window`` (``h`` keyed ``(i, 1, 0, step)``);
     its contexts are the entries up to ``r`` positions to either side, stopping at a boundary, in increasing
@@ -876,7 +876,17 @@ def w2v_window_fused(seq: torch.Tensor, pos: torch.Tensor, n_comp: torch.Tensor,
     ``w_in`` / ``w_out``: :class:`ShardTableC` of the same stride, at most 512 floats.  ``stats`` (float32 ``[2]``)
     accumulates ``sum -log sigmoid(+-d)`` and the targets trained, ``token_stats`` (int64 ``[4]``) the contexts at
     index 2, ``nan_flag`` is set by a non-finite ``d``.  ``reserve_total``: CTA slots left free for the replica
-    exchange running next to it."""
+    exchange running next to it.
+
+    CBOW, per kept center with ``cw >= 1`` contexts (the same windows): ``h`` is the mean of the contexts'
+    ``W_in`` rows as pulled.  The targets are the center word (label 1), then ``negative`` noise words drawn as
+    those of context slot 0 but rejected against the center word.  Per target ``d = h . v``,
+    ``g = lr (label - sigmoid(d))``; ``g h`` is pushed to ``W_out[t]`` at once and ``g v`` summed into ``e``.  ``e``
+    is then pushed, unscaled, to ``W_in`` of every context, once per occurrence (word2vec.c's rule: each context row
+    moves by ``-lr * cw`` times the loss gradient with respect to that row).  A center with no context trains nothing;
+    ``token_stats[2]`` counts the contexts."""
+    if not isinstance(cbow, bool):
+        raise ValueError(f"cbow must be True or False, got {cbow!r}")
     for t, name in ((seq, "seq"), (pos, "pos"), (n_comp, "n_comp")):
         _req(t, name, torch.int32)
     if int(w_in.stride) != int(w_out.stride):
@@ -908,7 +918,10 @@ def w2v_window_fused(seq: torch.Tensor, pos: torch.Tensor, n_comp: torch.Tensor,
         _req(nan_flag, "nan_flag", torch.int32)
         a.nan_flag = nan_flag.data_ptr()
     a.reserve_total = int(reserve_total)
-    _check(lib().fps_w2v_window_fused(C.byref(a), sm_count(seq.device.index), _stream()), "w2v_window_fused")
+    if cbow:
+        _check(lib().fps_w2v_cbow_fused(C.byref(a), sm_count(seq.device.index), _stream()), "w2v_cbow_fused")
+    else:
+        _check(lib().fps_w2v_window_fused(C.byref(a), sm_count(seq.device.index), _stream()), "w2v_window_fused")
     _bump()
 
 
