@@ -155,13 +155,15 @@ __device__ __forceinline__ void fps_mf_step_body(const MfArgs& a) {
         if (j == 0) {
           rt[r] = rating;
         } else {
-          // K5: device-side negative sample, rejecting the positive item itself.
+          // K5: device-side negative sample, rejecting the positive item itself.  The shift is reduced
+          // modulo num_items - 1 (the host requires num_items >= 2) so it never lands back on the positive.
           Philox4 s = fps_philox((uint32_t)pos, (uint32_t)((unsigned long long)pos >> 32),
                                  (uint32_t)j, (uint32_t)a.step, (uint32_t)a.seed,
                                  (uint32_t)(a.seed >> 32));
           unsigned long long h = ((unsigned long long)s.x << 32) | s.y;
           long long neg = (long long)(h % (unsigned long long)a.num_items);
-          if (neg == (long long)item) neg = (neg + 1 + (long long)(s.z % 7u)) % a.num_items;
+          if (neg == (long long)item)
+            neg = (neg + 1 + (long long)((s.z % 7u) % (unsigned long long)(a.num_items - 1))) % a.num_items;
           item = (IdT)neg;
         }
       }

@@ -16,7 +16,7 @@
 // Negatives come from an int tensor [n_pos, n] (-1 voids a triple) or are drawn in the kernel from
 // the K5 Philox stream of fps_mf_sgd_fused_kernel (key (pos, j, step, seed), uniform over
 // [0, num_items), the positive rejected by a shift of 1 + s.z % 7).  The shift is reduced modulo
-// num_items - 1 so that it never lands back on the positive: identical to K5 for num_items >= 8.
+// num_items - 1 so that it never lands back on the positive, as in every kernel that draws K5.
 //
 // Rows: the anchor rows and the candidate rows are each read either from a worker-local table
 // (slot = id / div) or through a ShardTable (local shard, NVLink peer shard, or a replica); the

@@ -92,6 +92,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1)
           }
           user[p] = users[pos];
           item[p] = items[pos];
+          if (user[p] < 0) ok[p] = false;  // record voided upstream (fps_neg_sample: no unseen item found)
           if (j == 0) rt[p] = a.ratings[pos];
           jj[p] = j; pp[p] = pos;
         }
@@ -110,7 +111,8 @@ __global__ void __launch_bounds__(TMA_THREADS, 1)
                                  (uint32_t)(a.seed >> 32));
           unsigned long long h = ((unsigned long long)s.x << 32) | s.y;
           long long neg = (long long)(h % (unsigned long long)a.num_items);
-          if (neg == (long long)item[p]) neg = (neg + 1 + (long long)(s.z % 7u)) % a.num_items;
+          if (neg == (long long)item[p])   // never back on the positive (fps_core.cu K5)
+            neg = (neg + 1 + (long long)((s.z % 7u) % (unsigned long long)(a.num_items - 1))) % a.num_items;
           item[p] = (IdT)neg;
         }
         float* up = a.user_sharded

@@ -239,6 +239,23 @@ def init_rows(rows: torch.Tensor, dim: int, shard: int, num_shards: int, mode: i
     _bump()
 
 
+MF_ERR_MODES = (0, 1, 2)   # the error rules of the pointwise step (fps_mf_args.cuh fps_mf_grad)
+
+
+def _check_pointwise(users, items, ratings, err_mode) -> None:
+    """Refusals shared by :func:`mf_sgd_fused` and :func:`mf_sgd_fused_f64` that need no device tensor."""
+    if int(err_mode) not in MF_ERR_MODES:
+        raise ValueError(f"err_mode must be one of {MF_ERR_MODES}, got {err_mode!r}")
+    if items is None:
+        if users.dtype != torch.int64:
+            raise TypeError("packed rating records must be an int64 tensor (see pack_ratings)")
+        return
+    if users.dtype != items.dtype:
+        raise TypeError("users and items must share an integer dtype")
+    if items.numel() != users.numel() or ratings.numel() != users.numel():
+        raise ValueError("users, items and ratings must have the same length")
+
+
 def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor,
                  user_table, user_div: int, item_tab: ShardTableC, lr: float,
                  err_mode: int = 0, neg_rate: int = 0, num_items: int = 0, seed: int = 0,
@@ -259,19 +276,21 @@ def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
     ``kernel="reg"`` (default): register-staged loads at full occupancy (csrc/fps_core.cu);
     ``kernel="tma"``: warp-specialised TMA/mbarrier pipeline (csrc/fps_mf_tma.cu) -- slower for
     256-byte rows, kept for large rows.
-    ``items=None`` means ``users`` holds packed64 records (see :func:`pack_ratings`)."""
+    ``items=None`` means ``users`` holds packed64 records (see :func:`pack_ratings`).
+
+    ``err_mode``: 0 ``e = sigmoid(r - u.v)``, 1 ``e = r - u.v``, 2 ``e = r - sigmoid(u.v)``.  ``neg_rate > 0``
+    draws that many negatives per record in the kernel, uniform over ``[0, num_items)`` and never the
+    positive, so it needs ``num_items >= 2``."""
+    _check_pointwise(users, items, ratings, err_mode)
+    if int(neg_rate) > 0 and int(num_items) < 2:
+        raise ValueError(f"sampled negatives need num_items >= 2, got {num_items}")
     _req(users, "users")
     user_sharded = isinstance(user_table, ShardTableC)
     if not user_sharded:
         _req(user_table, "user_table", torch.float32)
     packed = items is None
-    if packed:
-        if users.dtype != torch.int64:
-            raise TypeError("packed rating records must be an int64 tensor (see pack_ratings)")
-    else:
+    if not packed:
         _req(items, "items"); _req(ratings, "ratings", torch.float32)
-        if users.dtype != items.dtype:
-            raise TypeError("users and items must share an integer dtype")
     if (user_table.stride if user_sharded else user_table.shape[1]) != item_tab.stride:
         raise ValueError("user table stride must equal item table stride")
     a = MfArgsC()
@@ -470,6 +489,8 @@ def _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, neg
     else:
         if int(n_neg) < 1:
             raise ValueError("n_neg must be >= 1 when negatives are sampled")
+        if int(num_items) < 2:
+            raise ValueError(f"sampled negatives need num_items >= 2, got {num_items}")
         a.n_neg = int(n_neg)
     if stats is not None:
         _req(stats, "stats", torch.float32)
@@ -592,7 +613,9 @@ def mf_sgd_fused_f64(users: torch.Tensor, items: Optional[torch.Tensor], ratings
                      err_mode: int = 0, stats: Optional[torch.Tensor] = None,
                      nan_flag: Optional[torch.Tensor] = None) -> None:
     """fp64 fused pull + SGD + push (csrc/fps_mf_f64.cu): ``user_table`` is float64 ``[n, k_pad]``, the shards
-    of ``item_tab`` hold doubles (stride counted in 4-byte cells).  ``items=None``: packed64 records."""
+    of ``item_tab`` hold doubles (stride counted in 4-byte cells).  ``items=None``: packed64 records.
+    ``err_mode`` as for :func:`mf_sgd_fused`."""
+    _check_pointwise(users, items, ratings, err_mode)
     _req(users, "users"); _req(user_table, "user_table", torch.float64)
     packed = items is None
     if not packed:

@@ -118,12 +118,7 @@ def test_warp_learner_orientation_matches_reference(dev, cand_div, idt):
 
 def _bpr_negative0(pos, items, num_items, step, seed):
     """BPR's negative 0 of record ``pos`` (the K5 key (pos, 1, step, seed)), replayed with tests/philox_ref.py."""
-    pos = np.asarray(pos, dtype=np.int64)
-    x, y, z, _ = philox_ref.philox4x32(pos & 0xFFFFFFFF, pos >> 32, 1, step, seed & 0xFFFFFFFF, seed >> 32)
-    h = (x.astype(np.uint64) << np.uint64(32)) | y.astype(np.uint64)
-    neg = (h % np.uint64(num_items)).astype(np.int64)
-    shift = (1 + (z % 7).astype(np.int64) % (num_items - 1))
-    return np.where(neg == items, (neg + shift) % num_items, neg)
+    return philox_ref.k5_negative(pos, 1, items, num_items, step, seed)[0]
 
 
 def test_sampled_candidates_are_bprs_negatives(dev):
