@@ -247,7 +247,11 @@ __global__ void __launch_bounds__(256, MINB) fps_mf_bpr_adagrad_kernel(const __g
         d += u[c].x * (vi[c].x - vj[c].x) + u[c].y * (vi[c].y - vj[c].y) +
              u[c].z * (vi[c].z - vj[c].z) + u[c].w * (vi[c].w - vj[c].w);
       }
-      const float G_j = live ? fps_ld_f32(gjp) : 0.f;
+      // G_j is read by lane 0, which issued this row's earlier G += s, and shuffled to the group: a negative
+      // repeated in the list then reads G_j + s_j of its earlier triple on every lane (DESIGN §2.10).  A plain
+      // load on the other lanes is not ordered after lane 0's reduction.
+      float G_j = (live && lane == 0) ? fps_ld_f32(gjp) : 0.f;
+      G_j = __shfl_sync(0xffffffffu, G_j, 0, LPR);
       const float x = fps_group_sum<LPR>(d);
       const float g = 1.f / (1.f + __expf(x));   // sigmoid(-x)
       float n2 = 0.f;
