@@ -381,7 +381,8 @@ class WinArgsC(C.Structure):
 def mf_window_drain(stage: torch.Tensor, slot_bytes: int, counts, formats, user_table: torch.Tensor,
                     item_table: torch.Tensor, lr: float, err_mode: int, slots: torch.Tensor,
                     user_bits: torch.Tensor, ctl: torch.Tensor, stats: torch.Tensor, slot_stats: torch.Tensor,
-                    nan_flag: torch.Tensor, phase_ns: Optional[torch.Tensor] = None) -> None:
+                    nan_flag: torch.Tensor, phase_ns: Optional[torch.Tensor] = None,
+                    num_sms: Optional[int] = None) -> None:
     """Apply the micro-batches staged in ``stage`` (slot j at byte ``j * slot_bytes``: ``counts[j]`` records,
     ``formats[j]`` 1 = packed64, 0 = int32 users | int32 items | fp32 ratings) in order, in one cooperative
     launch (csrc/fps_mf_window.cu).  Conflict-free runs of micro-batches are applied item-major with the tables
@@ -390,10 +391,14 @@ def mf_window_drain(stage: torch.Tensor, slot_bytes: int, counts, formats, user_
     ``slot_stats``: float32 ``[>= n, 2]`` receives each micro-batch's (sum sq err, updates), ``stats`` the totals
     (``DeviceOnlineMF`` reads only the totals; the per-micro-batch sums serve callers that report per micro-batch).
     ``phase_ns``: optional int64 ``[4]``; the drain adds its build and apply nanoseconds to ``[0]`` and ``[1]`` and
-    the windows it applied to ``[2]`` (``[3]`` is scratch)."""
+    the windows it applied to ``[2]`` (``[3]`` is scratch).  ``num_sms``: SMs the cooperative grid is sized for
+    (default: the device's); a smaller grid runs more rounds of every grid-stride loop and computes the same
+    tables bitwise, since each item's chain is applied by one lane-group in micro-batch order."""
     n = len(counts)
     if not 0 < n <= WINDOW_MAX or len(formats) != n:
         raise ValueError(f"1..{WINDOW_MAX} staged micro-batches expected, got {n}")
+    if num_sms is not None and int(num_sms) < 1:
+        raise ValueError(f"num_sms must be >= 1, got {num_sms!r}")
     for t, name in ((stage, "stage"), (user_table, "user_table"), (item_table, "item_table"), (slots, "slots"),
                     (user_bits, "user_bits"), (ctl, "ctl"), (stats, "stats"), (slot_stats, "slot_stats"),
                     (nan_flag, "nan_flag")):
@@ -421,7 +426,9 @@ def mf_window_drain(stage: torch.Tensor, slot_bytes: int, counts, formats, user_
     rv = os.environ.get("FPS_MF_WINDOW_VARIANT")
     if rv is not None:
         lib().fps_set_mf_window_variant(int(rv))
-    _check(lib().fps_mf_window_drain(C.byref(a), sm_count(stage.device.index), _stream()), "mf_window_drain")
+    if num_sms is None:
+        num_sms = sm_count(stage.device.index)
+    _check(lib().fps_mf_window_drain(C.byref(a), int(num_sms), _stream()), "mf_window_drain")
     _bump()
 
 
