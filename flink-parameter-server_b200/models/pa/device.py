@@ -39,10 +39,33 @@ def algo_to_device(algo) -> Tuple[str, float, Optional[np.ndarray]]:
     raise TypeError(f"no device kernel for {type(algo).__name__}")
 
 
+MAX_LABELS = 1024  # PA_MAX_LABELS of ops/csrc/fps_pa.cu
+
+
+def labels_array(labels: Sequence[Optional[int]], binary: bool, num_labels: int) -> np.ndarray:
+    """The int32 label column of one micro-batch: ``None`` -> ``native.PA_UNLABELLED`` (predict only).
+    A binary label must be +1 or -1 and a class index must lie in ``[0, num_labels)``; anything else raises
+    ``ValueError``.  The kernels index their decision vector and the cost matrix with the label, and a
+    binary ``0`` (``int(False)``) would train towards no target at all."""
+    lab = np.array([native.PA_UNLABELLED if l is None else int(l) for l in labels], dtype=np.int64)
+    live = lab != native.PA_UNLABELLED
+    if binary:
+        wrong = live & (lab != 1) & (lab != -1)
+        what = "binary labels must be +1 or -1"
+    else:
+        wrong = live & ((lab < 0) | (lab >= num_labels))
+        what = f"class labels must lie in [0, {num_labels})"
+    if wrong.any():
+        raise ValueError(f"{what}; got {lab[wrong][:8].tolist()}")
+    return lab.astype(np.int32)
+
+
 class DevicePassiveAggressive:
     def __init__(self, feature_count: int, num_labels: int = 1, binary: bool = True, algo: str = "PA",
                  aggressiveness: float = 0.0, cost: Optional[np.ndarray] = None,
                  range_partitioning: bool = False, group=None, device: Optional[int] = None):
+        if not binary and not 1 <= int(num_labels) <= MAX_LABELS:
+            raise ValueError(f"num_labels must lie in [1, {MAX_LABELS}]; got {num_labels}")
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.dev = torch.device("cuda", self.device)
         self.binary, self.L, self.algo, self.C = binary, (1 if binary else num_labels), algo, aggressiveness
@@ -55,7 +78,9 @@ class DevicePassiveAggressive:
     def step_csr(self, row_ptr: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor,
                  labels: torch.Tensor) -> torch.Tensor:
         """One micro-batch; ``labels``: binary +-1 / class index / ``native.PA_UNLABELLED``.
-        Returns predictions (made with the parameters *before* each example's own update)."""
+        Returns predictions (made with the parameters *before* each example's own update).
+        The labels are not checked here (that would wait for the device): the caller guarantees +-1 for a
+        binary model and ``[0, num_labels)`` for a multiclass one.  :meth:`step` checks them."""
         pred = torch.empty(labels.numel(), dtype=torch.int32, device=self.dev)
         # mark every referenced feature as touched (what close() dumps)
         if self.table.track_touched:
@@ -66,14 +91,14 @@ class DevicePassiveAggressive:
         return pred
 
     def step(self, vectors: Sequence[SparseVector], labels: Sequence[Optional[int]]) -> List[int]:
+        """One micro-batch from the host; ``None`` labels only predict.  Refuses bad labels before any copy."""
+        lab = labels_array(labels, self.binary, self.L)
         n = len(vectors)
         row_ptr = np.zeros(n + 1, dtype=np.int64)
         for i, v in enumerate(vectors):
             row_ptr[i + 1] = row_ptr[i] + v.activeSize
         cols = np.concatenate([v.indices for v in vectors]).astype(np.int32) if n else np.zeros(0, np.int32)
         vals = np.concatenate([v.values for v in vectors]).astype(np.float32) if n else np.zeros(0, np.float32)
-        lab = np.array([native.PA_UNLABELLED if l is None else int(l) for l in labels], dtype=np.int64)
-        lab = lab.astype(np.int32)
         to = lambda x: torch.from_numpy(x).to(self.dev, non_blocking=True)
         pred = self.step_csr(to(row_ptr), to(cols), to(vals), to(lab))
         return pred.cpu().tolist()

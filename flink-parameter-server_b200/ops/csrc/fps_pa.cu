@@ -36,6 +36,16 @@ struct PaArgs {
   ShardTable tab;            // one row per feature: [stride >= L] floats
 };
 
+// Arg-max order of both kernels: (v, i) beats (best, arg) if v is larger, or equal with a lower index;
+// NaN ranks above every number.  This is np.argmax (first maximum, first NaN), it is a total order, so
+// every lane of a shuffle reduction ends on the same winner, and a seed of (-inf, INT_MAX) loses to
+// every real column, even when all of them are -inf.
+__device__ __forceinline__ bool pa_beats(float v, int i, float best, int arg) {
+  const bool vn = v != v, bn = best != best;
+  if (vn != bn) return vn;
+  return v > best || (!(v < best) && i < arg);
+}
+
 template <typename IdT, int LPR>
 __global__ void __launch_bounds__(PA_THREADS)
     fps_pa_step_kernel(const __grid_constant__ PaArgs a) {
@@ -93,7 +103,7 @@ __global__ void __launch_bounds__(PA_THREADS)
       int arg = 0;
       float best = s_dec[0];
       for (int i = 1; i < L; ++i)
-        if (s_dec[i] > best) { best = s_dec[i]; arg = i; }
+        if (pa_beats(s_dec[i], i, best, arg)) { best = s_dec[i]; arg = i; }
       a.pred[ex] = a.binary ? (s_dec[0] > 0.f ? 1 : 0) : arg;
       s_aux[0] = arg;
       s_aux[1] = -1;
@@ -120,11 +130,12 @@ __global__ void __launch_bounds__(PA_THREADS)
         if (threadIdx.x == 0) {
           int q = s_aux[0];
           if (a.algo == PA_ML) {
-            float bestv = -3.0e38f;
+            float bestv = -INFINITY;
+            q = 0x7fffffff;
             for (int i = 0; i < L; ++i) {
               const float c = a.cost ? a.cost[label * L + i] : (i == label ? 0.f : 1.f);
               const float v = s_dec[i] - s_dec[label] + sqrtf(c);
-              if (v > bestv) { bestv = v; q = i; }
+              if (pa_beats(v, i, bestv, q)) { bestv = v; q = i; }
             }
           }
           float tau = 0.f;
@@ -161,7 +172,8 @@ __global__ void __launch_bounds__(PA_THREADS)
             d.z = (4 * q + 2 < L) ? x * s_dec[4 * q + 2] : 0.f;
             d.w = (4 * q + 3 < L) ? x * s_dec[4 * q + 3] : 0.f;
             if (d.x != 0.f || d.y != 0.f || d.z != 0.f || d.w != 0.f) {
-              if (!(fabsf(d.x) <= 3.0e38f)) bad = true;
+              // all four columns, like the warp kernel: one inf or NaN anywhere in the chunk flags it
+              if (!(fabsf(d.x) + fabsf(d.y) + fabsf(d.z) + fabsf(d.w) <= 3.0e38f)) bad = true;
               fps_red_add4(row + 4 * q, d);  // the PUSH fused with paramUpdate (+)
             }
           }
@@ -186,15 +198,15 @@ __device__ __forceinline__ float pa_sel4(const float4& v, int i) {
 __device__ __forceinline__ void pa_red_add1(float* p, float v) {
   asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
 }
-// (value, index) arg-max over the LPR lanes of a group; ties -> lowest index (first maximum wins, like
-// the sequential scans of the host algorithms)
+// (value, index) arg-max over the LPR lanes of a group in pa_beats order (first maximum wins, like the
+// sequential scans of the host algorithms)
 template <int LPR>
 __device__ __forceinline__ void pa_group_argmax(float& v, int& idx) {
 #pragma unroll
   for (int o = LPR / 2; o > 0; o >>= 1) {
     const float ov = __shfl_xor_sync(0xffffffffu, v, o);
     const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-    if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
+    if (pa_beats(ov, oi, v, idx)) { v = ov; idx = oi; }
   }
 }
 // component `label` of the distributed decision vector, broadcast to every lane
@@ -252,12 +264,13 @@ __global__ void __launch_bounds__(256, 4) fps_pa_step_warp_kernel(const __grid_c
     }
     // ---- phase 2: prediction + multipliers ---------------------------------------------------
     const int label = a.labels[ex];
-    float best = -3.0e38f;
+    // the seed loses to every column, -inf and NaN included; a lane past L keeps it and loses the reduction
+    float best = -INFINITY;
     int arg = 0x7fffffff;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float v = pa_sel4(dec, i);
-      if (4 * q + i < L && v > best) { best = v; arg = 4 * q + i; }
+      if (4 * q + i < L && pa_beats(v, 4 * q + i, best, arg)) { best = v; arg = 4 * q + i; }
     }
     pa_group_argmax<LPR>(best, arg);
     if (lane == 0) a.pred[ex] = a.binary ? (best > 0.f ? 1 : 0) : arg;
@@ -287,7 +300,7 @@ __global__ void __launch_bounds__(256, 4) fps_pa_step_warp_kernel(const __grid_c
       int qq = arg;
       const float d_label = pa_group_get<LPR>(dec, label, lane);
       if (a.algo == PA_ML) {
-        float bestv = -3.0e38f;
+        float bestv = -INFINITY;
         int bi = 0x7fffffff;
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
@@ -295,7 +308,7 @@ __global__ void __launch_bounds__(256, 4) fps_pa_step_warp_kernel(const __grid_c
           if (li < L) {
             const float c = a.cost ? a.cost[label * L + li] : (li == label ? 0.f : 1.f);
             const float v = pa_sel4(dec, i) - d_label + sqrtf(c);
-            if (v > bestv) { bestv = v; bi = li; }
+            if (pa_beats(v, li, bestv, bi)) { bestv = v; bi = li; }
           }
         }
         pa_group_argmax<LPR>(bestv, bi);
