@@ -13,7 +13,6 @@
 // One cooperative kernel, no host synchronisation (fps_bucket_deal_kernel below): a histogram over the bucket
 // ids, a grid sync, then a scatter in which each CTA reserves one contiguous run per bucket (shared-memory ranks
 // + one global atomic per (CTA, bucket)).  Cost: read the batch from HBM once and from L2 once, write it once.
-#include <cuda_fp16.h>
 #include <cooperative_groups.h>
 #include "fps_common.cuh"
 
@@ -42,8 +41,10 @@ struct BucketArgs {
 };
 
 __device__ __forceinline__ long long bk_item(const BucketArgs& a, long long i) {
+  // not fps_record_item: its two instantiations behind a runtime id width cost this kernel 144 instructions
   if (a.format == 1)
-    return (long long)((reinterpret_cast<const unsigned long long*>(a.users)[i] >> 16) & 0x3FFFFFull);
+    return (long long)((reinterpret_cast<const unsigned long long*>(a.users)[i] >> FPS_REC_ITEM_SHIFT) &
+                       FPS_REC_ITEM_MASK);
   if (a.id_bytes == 8) return reinterpret_cast<const long long*>(a.items)[i];
   return (long long)reinterpret_cast<const int*>(a.items)[i];
 }

@@ -6,6 +6,7 @@
 // pull is a load through base[owner(id)], a push is a red.add through the same pointer:
 // there are no messages on the hot path (SURVEY §5.8; replaces FPS:411-463 routing).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -176,6 +177,62 @@ __host__ __device__ __forceinline__ Philox4 fps_philox(uint32_t c0, uint32_t c1,
 }
 __host__ __device__ __forceinline__ float fps_u01(uint32_t x) {
   return (float)(x >> 8) * (1.0f / 16777216.0f);
+}
+
+// K5: in-kernel negative `j` of record `pos`, uniform over [0, a.num_items) from the Philox stream keyed
+// (pos, j, a.step, a.seed).  A draw equal to the positive is shifted by 1 + s.z % 7, reduced modulo
+// num_items - 1 so that it never lands back on the positive (num_items >= 2).  `a` is the kernel's argument
+// block (MfArgs, BprArgs): step, seed and num_items are read where the draw uses them, which keeps every
+// kernel's machine code as it was when each spelled the draw out.
+template <typename Args, typename IdT>
+__device__ __forceinline__ long long fps_k5_negative(const Args& a, long long pos, int j, IdT positive) {
+  const Philox4 s = fps_philox((uint32_t)pos, (uint32_t)((unsigned long long)pos >> 32), (uint32_t)j,
+                               (uint32_t)a.step, (uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+  const unsigned long long h = ((unsigned long long)s.x << 32) | s.y;
+  long long neg = (long long)(h % (unsigned long long)a.num_items);
+  if (neg == (long long)positive)
+    neg = (neg + 1 + (long long)((s.z % 7u) % (unsigned long long)(a.num_items - 1))) % a.num_items;
+  return neg;
+}
+
+// ---- training records ---------------------------------------------------------------------------------------
+// A batch is either packed64 records in `users` (format 1: user:26 | item:22 | fp16 rating:16, 8 B per update)
+// or users / items / ratings arrays of IdT ids (format 0).  The host packs with the same layout
+// (ops/native.py pack_ratings, fps_host.cpp).  Which records are void is the caller's rule.
+constexpr int FPS_REC_USER_SHIFT = 38;
+constexpr int FPS_REC_ITEM_SHIFT = 16;
+constexpr unsigned long long FPS_REC_ITEM_MASK = 0x3FFFFFull;
+
+// Record i with its ids as OutT.  Returned by value, rating first: a decoder writing through reference parameters,
+// or this struct with the ids first, changed the code nvcc generates for the pointwise and BPR kernels.
+template <typename OutT>
+struct FpsRecord {
+  float rating;
+  OutT user, item;
+};
+template <typename IdT, typename OutT = IdT>
+__device__ __forceinline__ FpsRecord<OutT> fps_record(int format, const void* users, const void* items,
+                                                      const float* ratings, long long i) {
+  FpsRecord<OutT> r;
+  if (format == 1) {
+    const unsigned long long rec = reinterpret_cast<const unsigned long long*>(users)[i];
+    r.user = (OutT)(rec >> FPS_REC_USER_SHIFT);
+    r.item = (OutT)((rec >> FPS_REC_ITEM_SHIFT) & FPS_REC_ITEM_MASK);
+    r.rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
+  } else {
+    r.user = (OutT)reinterpret_cast<const IdT*>(users)[i];
+    r.item = (OutT)reinterpret_cast<const IdT*>(items)[i];
+    r.rating = ratings[i];
+  }
+  return r;
+}
+// The item of record i alone.
+template <typename IdT>
+__device__ __forceinline__ long long fps_record_item(int format, const void* users, const void* items, long long i) {
+  if (format == 1)
+    return (long long)((reinterpret_cast<const unsigned long long*>(users)[i] >> FPS_REC_ITEM_SHIFT) &
+                       FPS_REC_ITEM_MASK);
+  return (long long)reinterpret_cast<const IdT*>(items)[i];
 }
 
 // Warp-subgroup all-reduce (sum) over LPR consecutive lanes (LPR power of two <= 32).

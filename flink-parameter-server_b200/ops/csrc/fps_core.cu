@@ -7,7 +7,6 @@
 // Reference behaviour being reproduced (not code): SimplePSLogic.scala:13-25 (init on
 // first pull, additive update), SGDUpdater.scala:5-14 (delta rule),
 // PSOnlineMatrixFactorizationWorker.scala:42-89 (worker step + negative sampling).
-#include <cuda_fp16.h>
 #include "fps_common.cuh"
 #include "fps_mf_args.cuh"
 
@@ -108,6 +107,8 @@ __device__ __forceinline__ void fps_mf_step_body(const MfArgs& a) {
   const long long n_eff = a.n_pos * per_pos;
   const int stride = a.item_tab.stride;
   const int nvec = stride >> 2;
+  // the id arrays are read through these (packed records through a.users): with the record pointers taken from
+  // `a` at the decode, nvcc orders this kernel's argument loads differently
   const IdT* __restrict__ users = reinterpret_cast<const IdT*>(a.users);
   const IdT* __restrict__ items = reinterpret_cast<const IdT*>(a.items);
   float sq_acc = 0.f, cnt_acc = 0.f;
@@ -140,32 +141,14 @@ __device__ __forceinline__ void fps_mf_step_body(const MfArgs& a) {
       IdT user = 0, item = 0;
       rt[r] = 0.f;
       if (ok[r]) {
-        float rating;
-        if (FMT == 1) {
-          const unsigned long long rec = reinterpret_cast<const unsigned long long*>(a.users)[pos];
-          user = (IdT)(rec >> 38);
-          item = (IdT)((rec >> 16) & 0x3FFFFFull);
-          rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
-        } else {
-          user = users[pos];
-          item = items[pos];
-          rating = a.ratings[pos];
-          if (user < 0) ok[r] = false;  // record voided upstream (fps_neg_sample: no unseen item found)
-        }
-        if (j == 0) {
-          rt[r] = rating;
-        } else {
-          // K5: device-side negative sample, rejecting the positive item itself.  The shift is reduced
-          // modulo num_items - 1 (the host requires num_items >= 2) so it never lands back on the positive.
-          Philox4 s = fps_philox((uint32_t)pos, (uint32_t)((unsigned long long)pos >> 32),
-                                 (uint32_t)j, (uint32_t)a.step, (uint32_t)a.seed,
-                                 (uint32_t)(a.seed >> 32));
-          unsigned long long h = ((unsigned long long)s.x << 32) | s.y;
-          long long neg = (long long)(h % (unsigned long long)a.num_items);
-          if (neg == (long long)item)
-            neg = (neg + 1 + (long long)((s.z % 7u) % (unsigned long long)(a.num_items - 1))) % a.num_items;
-          item = (IdT)neg;
-        }
+        const FpsRecord<IdT> rec = fps_record<IdT>(FMT, FMT == 1 ? a.users : users, items, a.ratings, pos);
+        user = rec.user;
+        item = rec.item;
+        const float rating = rec.rating;
+        if (FMT == 0 && user < 0) ok[r] = false;  // record voided upstream (fps_neg_sample: no unseen item found)
+        // j > 0: the K5 negative (the host requires num_items >= 2)
+        if (j == 0) rt[r] = rating;
+        else item = (IdT)fps_k5_negative(a, pos, j, item);
       }
       uid[r] = (long long)user;
       if (LIMIT) {
@@ -300,35 +283,16 @@ __global__ void __launch_bounds__(256, MINB)
   fps_mf_step_body<IdT, LPR, VPL, R, FMT, 0, 0, 0, 1>(a);
 }
 
-static int g_mf_reserve = 0;        // CTA slots per SM left free for a concurrently running kernel
-static int g_mf_reserve_total = 0;  // CTA slots left free on the whole GPU (the replica exchange CTAs)
-extern "C" void fps_set_mf_reserve(int v) { g_mf_reserve = v < 0 ? 0 : v; }
-extern "C" void fps_set_mf_reserve_total(int v) { g_mf_reserve_total = v < 0 ? 0 : v; }
-
+// A lane-group keeps R records, and so R row pairs, in flight.
 template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT, int HINT = 0, int EMIT = 0, int LIMIT = 0,
           int ADA = 0>
 static int launch_mf(const MfArgs& a, int max_inflight_rows, int num_sms, cudaStream_t stream) {
   const int threads = 256;
-  const int groups_per_block = threads / LPR;
   void (*kern)(const MfArgs);
   if constexpr (ADA) kern = fps_mf_adagrad_fused_kernel<IdT, LPR, VPL, R, MINB, FMT>;
   else kern = fps_mf_sgd_fused_kernel<IdT, LPR, VPL, R, MINB, FMT, HINT, EMIT, LIMIT>;
-  int occ = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, 0);
-  occ -= g_mf_reserve;  // leave slots for the background replica exchange (see fps_cache_sync)
-  if (occ < 1) occ = 1;
-  long long blocks = (long long)num_sms * occ - g_mf_reserve_total;
-  if (blocks < num_sms) blocks = num_sms;
-  // pull limiter: rows in flight = blocks * groups_per_block * R  <=  pullLimit
-  if (max_inflight_rows > 0) {
-    long long cap = max_inflight_rows / ((long long)groups_per_block * R);
-    if (cap < 1) cap = 1;
-    if (blocks > cap) blocks = cap;
-  }
-  const long long n_eff = a.n_pos * (1 + a.neg_rate);
-  long long need = (n_eff + (long long)groups_per_block * R - 1) / ((long long)groups_per_block * R);
-  if (need < 1) need = 1;
-  if (blocks > need) blocks = need;
+  const long long blocks = fps_row_grid(kern, threads, threads / LPR, num_sms, a.reserve_total, max_inflight_rows, R,
+                                        a.n_pos * (1 + a.neg_rate), R);
   kern<<<(int)blocks, threads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
@@ -399,10 +363,10 @@ static int dispatch_mf(const MfArgs& a, int max_inflight, int num_sms, cudaStrea
 extern "C" int fps_mf_sgd_fused(const MfArgs* args, int id_bytes, int max_inflight_rows,
                                 int num_sms, cudaStream_t stream) {
   if (args->n_pos <= 0) return 0;
-  if (args->format == 1) return dispatch_mf<int, 1>(*args, max_inflight_rows, num_sms, stream);
-  if (id_bytes == 4) return dispatch_mf<int, 0>(*args, max_inflight_rows, num_sms, stream);
-  if (id_bytes == 8) return dispatch_mf<long long, 0>(*args, max_inflight_rows, num_sms, stream);
-  return -1001;
+  return fps_with_id_form(args->format, id_bytes, [&](auto form) {
+    using F = decltype(form);
+    return dispatch_mf<typename F::Id, F::fmt>(*args, max_inflight_rows, num_sms, stream);
+  });
 }
 
 // ----------------------------------------------------------------------------------------

@@ -2,6 +2,7 @@
 // fps_mf_tma.cu TMA-pipelined kernel).  Mirrored by ops/native.py::MfArgsC.
 #pragma once
 #include "fps_common.cuh"
+#include "fps_launch.cuh"
 
 struct MfArgs {
   const void* users;
@@ -39,7 +40,7 @@ struct MfArgs {
   const unsigned long long* out_staged;
   long long out_cap;
   int out_every;             // 0 = no output stream
-  int pad3_;
+  int reserve_total;         // CTA slots left free on the whole GPU (the replica exchange CTAs)
   int* credits;              // device-side pull limiter (WL:196-250): credits[0] = pulls that may still be
                              //   issued, credits[1] = stall counter; nullptr = unlimited
   // Row-wise AdaGrad (one fp32 accumulator per row, partitioned like its table; stride 1).

@@ -25,7 +25,6 @@
 //
 // Row-wise AdaGrad (fps_mf_bpr_adagrad_kernel, DESIGN §2.10): the same deltas with lr = 1, each row
 // stepped by lr / (sqrt(G + |delta|^2 / k) + eps) with G its accumulator as pulled, and G += |delta|^2 / k.
-#include <cuda_fp16.h>
 #include "fps_common.cuh"
 #include "fps_mf_args.cuh"
 
@@ -50,17 +49,10 @@ __global__ void __launch_bounds__(256, MINB) fps_mf_bpr_kernel(const __grid_cons
     bool ok = pos < a.n_pos;
     IdT anchor = 0, item = 0;
     if (ok) {
-      float rating;
-      if (FMT == 1) {
-        const unsigned long long rec = reinterpret_cast<const unsigned long long*>(a.users)[pos];
-        anchor = (IdT)(rec >> 38);
-        item = (IdT)((rec >> 16) & 0x3FFFFFull);
-        rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
-      } else {
-        anchor = reinterpret_cast<const IdT*>(a.users)[pos];
-        item = reinterpret_cast<const IdT*>(a.items)[pos];
-        rating = a.ratings[pos];
-      }
+      const FpsRecord<IdT> rec = fps_record<IdT>(FMT, a.users, a.items, a.ratings, pos);
+      anchor = rec.user;
+      item = rec.item;
+      const float rating = rec.rating;
       // rating <= 0 (a pointwise stream's explicit negatives) and voided records are not positives
       ok = rating > 0.f && anchor >= 0 && item >= 0;
     }
@@ -88,15 +80,8 @@ __global__ void __launch_bounds__(256, MINB) fps_mf_bpr_kernel(const __grid_cons
       if (ok) {
         if (negs != nullptr) {
           neg = (long long)negs[pos * a.n_neg + j];
-        } else if (a.num_items > 1) {
-          // K5 stream of the pointwise kernel: record pos, negative number j + 1
-          Philox4 s = fps_philox((uint32_t)pos, (uint32_t)((unsigned long long)pos >> 32),
-                                 (uint32_t)(j + 1), (uint32_t)a.step, (uint32_t)a.seed,
-                                 (uint32_t)(a.seed >> 32));
-          const unsigned long long h = ((unsigned long long)s.x << 32) | s.y;
-          neg = (long long)(h % (unsigned long long)a.num_items);
-          if (neg == (long long)item)
-            neg = (neg + 1 + (long long)((s.z % 7u) % (unsigned long long)(a.num_items - 1))) % a.num_items;
+        } else if (a.num_items > 1) {   // K5 stream of the pointwise kernel: record pos, negative number j + 1
+          neg = fps_k5_negative(a, pos, j + 1, item);
         }
         if (neg == (long long)item) neg = -1;   // an explicit negative equal to the positive is void
       }
@@ -183,17 +168,10 @@ __global__ void __launch_bounds__(256, MINB) fps_mf_bpr_adagrad_kernel(const __g
     bool ok = pos < a.n_pos;
     IdT anchor = 0, item = 0;
     if (ok) {
-      float rating;
-      if (FMT == 1) {
-        const unsigned long long rec = reinterpret_cast<const unsigned long long*>(a.users)[pos];
-        anchor = (IdT)(rec >> 38);
-        item = (IdT)((rec >> 16) & 0x3FFFFFull);
-        rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
-      } else {
-        anchor = reinterpret_cast<const IdT*>(a.users)[pos];
-        item = reinterpret_cast<const IdT*>(a.items)[pos];
-        rating = a.ratings[pos];
-      }
+      const FpsRecord<IdT> rec = fps_record<IdT>(FMT, a.users, a.items, a.ratings, pos);
+      anchor = rec.user;
+      item = rec.item;
+      const float rating = rec.rating;
       ok = rating > 0.f && anchor >= 0 && item >= 0;
     }
     float* up = bpr_row<IdT>(a.anchor_table, a.anchor_div, a.anchor_shift, a.anchor_sharded,
@@ -225,13 +203,7 @@ __global__ void __launch_bounds__(256, MINB) fps_mf_bpr_adagrad_kernel(const __g
         if (negs != nullptr) {
           neg = (long long)negs[pos * a.n_neg + j];
         } else if (a.num_items > 1) {
-          Philox4 s = fps_philox((uint32_t)pos, (uint32_t)((unsigned long long)pos >> 32),
-                                 (uint32_t)(j + 1), (uint32_t)a.step, (uint32_t)a.seed,
-                                 (uint32_t)(a.seed >> 32));
-          const unsigned long long h = ((unsigned long long)s.x << 32) | s.y;
-          neg = (long long)(h % (unsigned long long)a.num_items);
-          if (neg == (long long)item)
-            neg = (neg + 1 + (long long)((s.z % 7u) % (unsigned long long)(a.num_items - 1))) % a.num_items;
+          neg = fps_k5_negative(a, pos, j + 1, item);
         }
         if (neg == (long long)item) neg = -1;
       }
@@ -335,23 +307,11 @@ __global__ void __launch_bounds__(256, MINB) fps_mf_bpr_adagrad_kernel(const __g
 template <typename IdT, int LPR, int VPL, int MINB, int FMT, int ADA = 0>
 static int launch_bpr(const BprArgs& a, int max_inflight_rows, int num_sms, cudaStream_t stream) {
   const int threads = 256;
-  const int groups_per_block = threads / LPR;
   void (*kern)(const BprArgs);
   if constexpr (ADA) kern = fps_mf_bpr_adagrad_kernel<IdT, LPR, VPL, MINB, FMT>;
   else kern = fps_mf_bpr_kernel<IdT, LPR, VPL, MINB, FMT>;
-  int occ = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, 0);
-  if (occ < 1) occ = 1;
-  long long blocks = (long long)num_sms * occ - a.reserve_total;
-  if (blocks < num_sms) blocks = num_sms;
-  if (max_inflight_rows > 0) {
-    long long cap = max_inflight_rows / (3LL * groups_per_block);
-    if (cap < 1) cap = 1;
-    if (blocks > cap) blocks = cap;
-  }
-  long long need = (a.n_pos + groups_per_block - 1) / groups_per_block;
-  if (need < 1) need = 1;
-  if (blocks > need) blocks = need;
+  const long long blocks = fps_row_grid(kern, threads, threads / LPR, num_sms, a.reserve_total, max_inflight_rows, 3,
+                                        a.n_pos, 1);
   kern<<<(int)blocks, threads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
@@ -389,8 +349,8 @@ extern "C" int fps_mf_bpr_fused(const BprArgs* args, int id_bytes, int max_infli
                                 cudaStream_t stream) {
   if (args->n_pos <= 0 || args->n_neg <= 0) return 0;
   if ((args->stride & 3) != 0) return -1000;
-  if (args->format == 1) return dispatch_bpr<int, 1>(*args, max_inflight_rows, num_sms, stream);
-  if (id_bytes == 4) return dispatch_bpr<int, 0>(*args, max_inflight_rows, num_sms, stream);
-  if (id_bytes == 8) return dispatch_bpr<long long, 0>(*args, max_inflight_rows, num_sms, stream);
-  return -1001;
+  return fps_with_id_form(args->format, id_bytes, [&](auto form) {
+    using F = decltype(form);
+    return dispatch_bpr<typename F::Id, F::fmt>(*args, max_inflight_rows, num_sms, stream);
+  });
 }

@@ -7,7 +7,6 @@
 // no vector form of the fp64 reduction), user update = local red.global.add.f64.  Same update rules as
 // fps_core.cu (SGDUpdater.scala:5-14).  Twice the bytes per update of the fp32 kernel: it runs at about
 // half its updates/s on the same memory system.
-#include <cuda_fp16.h>
 #include "fps_common.cuh"
 #include "fps_mf_args.cuh"
 
@@ -39,10 +38,12 @@ __global__ void __launch_bounds__(256, 4) fps_mf_sgd_fused_f64_kernel(const __gr
     double rating = 0.0;
     bool ok = in;
     if (in) {
+      // not fps_record: with it nvcc contracts this kernel's dot u.x*v.x + u.y*v.y the other way round in some
+      // instantiations (an fp64 rounding change)
       if (FMT == 1) {
         const unsigned long long rec = reinterpret_cast<const unsigned long long*>(a.users)[idx];
-        user = (IdT)(rec >> 38);
-        item = (IdT)((rec >> 16) & 0x3FFFFFull);
+        user = (IdT)(rec >> FPS_REC_USER_SHIFT);
+        item = (IdT)((rec >> FPS_REC_ITEM_SHIFT) & FPS_REC_ITEM_MASK);
         rating = (double)__half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
       } else {
         user = users[idx];
@@ -101,15 +102,11 @@ __global__ void __launch_bounds__(256, 4) fps_mf_sgd_fused_f64_kernel(const __gr
   if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
 }
 
+// No reserve and no pull limit: the fp64 step runs alone.
 template <typename IdT, int LPR, int VPL, int FMT>
 static int launch_f64(const MfArgs& a, int num_sms, cudaStream_t stream) {
-  int occ = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fps_mf_sgd_fused_f64_kernel<IdT, LPR, VPL, FMT>, 256, 0);
-  if (occ < 1) occ = 1;
-  long long blocks = (long long)num_sms * occ;
-  const long long per_block = 256 / LPR;
-  long long need = (a.n_pos + per_block - 1) / per_block;
-  if (blocks > need) blocks = need < 1 ? 1 : need;
+  const long long blocks = fps_row_grid(fps_mf_sgd_fused_f64_kernel<IdT, LPR, VPL, FMT>, 256, 256 / LPR, num_sms, 0, 0,
+                                        1, a.n_pos, 1);
   fps_mf_sgd_fused_f64_kernel<IdT, LPR, VPL, FMT><<<(int)blocks, 256, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
@@ -132,10 +129,10 @@ extern "C" int fps_mf_sgd_fused_f64(const MfArgs* args, int id_bytes, int num_sm
   if (args->n_pos <= 0) return 0;
   if (args->neg_rate != 0 || args->user_sharded || args->use_push_tab || args->out_every > 0 || args->credits != nullptr)
     return -1004;
-  if (args->format == 1) return dispatch_f64<int, 1>(*args, num_sms, stream);
-  if (id_bytes == 4) return dispatch_f64<int, 0>(*args, num_sms, stream);
-  if (id_bytes == 8) return dispatch_f64<long long, 0>(*args, num_sms, stream);
-  return -1001;
+  return fps_with_id_form(args->format, id_bytes, [&](auto form) {
+    using F = decltype(form);
+    return dispatch_f64<typename F::Id, F::fmt>(*args, num_sms, stream);
+  });
 }
 
 // K4 for fp64 rows: value(id, j) = lo + (hi - lo) * u53(philox(id, j / 2; seed)[2 * (j % 2) .. +1])

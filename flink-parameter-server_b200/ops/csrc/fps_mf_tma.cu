@@ -104,17 +104,8 @@ __global__ void __launch_bounds__(TMA_THREADS, 1)
         if (t >= n_tiles) break;
         const int stage = (int)(k % n_stages);
         const uint32_t phase = (uint32_t)((k / n_stages) & 1);
-        if (ok[p] && jj[p] != 0) {  // K5: device-side negative sample
-          const long long pos = pp[p];
-          Philox4 s = fps_philox((uint32_t)pos, (uint32_t)((unsigned long long)pos >> 32),
-                                 (uint32_t)jj[p], (uint32_t)a.step, (uint32_t)a.seed,
-                                 (uint32_t)(a.seed >> 32));
-          unsigned long long h = ((unsigned long long)s.x << 32) | s.y;
-          long long neg = (long long)(h % (unsigned long long)a.num_items);
-          if (neg == (long long)item[p])   // never back on the positive (fps_core.cu K5)
-            neg = (neg + 1 + (long long)((s.z % 7u) % (unsigned long long)(a.num_items - 1))) % a.num_items;
-          item[p] = (IdT)neg;
-        }
+        if (ok[p] && jj[p] != 0)  // K5: device-side negative sample
+          item[p] = (IdT)fps_k5_negative(a, pp[p], jj[p], item[p]);
         float* up = a.user_sharded
                         ? fps_row_t<IdT>(a.user_tab, user[p])
                         : a.user_table + fps_user_slot<IdT>(user[p], a.user_div, a.user_shift) * (size_t)stride;

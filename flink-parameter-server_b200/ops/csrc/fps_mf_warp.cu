@@ -20,7 +20,6 @@
 // each x_t is the same expression whatever the block it sits in, the result is bitwise independent of C.
 // The trial loop runs until every lane-group of the warp is done (__any_sync): fps_group_sum shuffles with a
 // full-warp mask, so a finished group keeps taking part with its loads and pushes predicated off.
-#include <cuda_fp16.h>
 #include "fps_common.cuh"
 #include "fps_mf_args.cuh"
 
@@ -43,17 +42,10 @@ __global__ void __launch_bounds__(256, MINB) fps_mf_warp_kernel(const __grid_con
     bool ok = pos < a.n_pos;
     IdT anchor = 0, item = 0;
     if (ok) {
-      float rating;
-      if (FMT == 1) {
-        const unsigned long long rec = reinterpret_cast<const unsigned long long*>(a.users)[pos];
-        anchor = (IdT)(rec >> 38);
-        item = (IdT)((rec >> 16) & 0x3FFFFFull);
-        rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
-      } else {
-        anchor = reinterpret_cast<const IdT*>(a.users)[pos];
-        item = reinterpret_cast<const IdT*>(a.items)[pos];
-        rating = a.ratings[pos];
-      }
+      const FpsRecord<IdT> rec = fps_record<IdT>(FMT, a.users, a.items, a.ratings, pos);
+      anchor = rec.user;
+      item = rec.item;
+      const float rating = rec.rating;
       ok = rating > 0.f && anchor >= 0 && item >= 0;
     }
     float* up = bpr_row<IdT>(a.anchor_table, a.anchor_div, a.anchor_shift, a.anchor_sharded,
@@ -89,15 +81,8 @@ __global__ void __launch_bounds__(256, MINB) fps_mf_warp_kernel(const __grid_con
         if (active && t < T) {
           if (negs != nullptr) {
             neg = (long long)negs[pos * T + t];
-          } else if (a.num_items > 1) {
-            // BPR's negative t: the K5 stream of the pointwise kernel, record pos, negative number t + 1
-            Philox4 s = fps_philox((uint32_t)pos, (uint32_t)((unsigned long long)pos >> 32),
-                                   (uint32_t)(t + 1), (uint32_t)a.step, (uint32_t)a.seed,
-                                   (uint32_t)(a.seed >> 32));
-            const unsigned long long h = ((unsigned long long)s.x << 32) | s.y;
-            neg = (long long)(h % (unsigned long long)a.num_items);
-            if (neg == (long long)item)
-              neg = (neg + 1 + (long long)((s.z % 7u) % (unsigned long long)(a.num_items - 1))) % a.num_items;
+          } else if (a.num_items > 1) {   // BPR's negative t: K5, record pos, negative number t + 1
+            neg = fps_k5_negative(a, pos, t + 1, item);
           }
           if (neg == (long long)item) neg = -1;
         }
@@ -184,21 +169,9 @@ __global__ void __launch_bounds__(256, MINB) fps_mf_warp_kernel(const __grid_con
 template <typename IdT, int LPR, int VPL, int MINB, int FMT, int C>
 static int launch_warp(const BprArgs& a, int max_inflight_rows, int num_sms, cudaStream_t stream) {
   const int threads = 256;
-  const int groups_per_block = threads / LPR;
   void (*kern)(const BprArgs) = fps_mf_warp_kernel<IdT, LPR, VPL, MINB, FMT, C>;
-  int occ = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, 0);
-  if (occ < 1) occ = 1;
-  long long blocks = (long long)num_sms * occ - a.reserve_total;
-  if (blocks < num_sms) blocks = num_sms;
-  if (max_inflight_rows > 0) {
-    long long cap = max_inflight_rows / ((2LL + C) * groups_per_block);
-    if (cap < 1) cap = 1;
-    if (blocks > cap) blocks = cap;
-  }
-  long long need = (a.n_pos + groups_per_block - 1) / groups_per_block;
-  if (need < 1) need = 1;
-  if (blocks > need) blocks = need;
+  const long long blocks = fps_row_grid(kern, threads, threads / LPR, num_sms, a.reserve_total, max_inflight_rows,
+                                        2 + C, a.n_pos, 1);
   kern<<<(int)blocks, threads, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }
@@ -241,8 +214,8 @@ extern "C" int fps_mf_warp_fused(const BprArgs* args, int id_bytes, int trial_bl
                                  int num_sms, cudaStream_t stream) {
   if (args->n_pos <= 0 || args->n_neg <= 0) return 0;
   if ((args->stride & 3) != 0) return -1000;
-  if (args->format == 1) return dispatch_warp<int, 1>(*args, trial_block, max_inflight_rows, num_sms, stream);
-  if (id_bytes == 4) return dispatch_warp<int, 0>(*args, trial_block, max_inflight_rows, num_sms, stream);
-  if (id_bytes == 8) return dispatch_warp<long long, 0>(*args, trial_block, max_inflight_rows, num_sms, stream);
-  return -1001;
+  return fps_with_id_form(args->format, id_bytes, [&](auto form) {
+    using F = decltype(form);
+    return dispatch_warp<typename F::Id, F::fmt>(*args, trial_block, max_inflight_rows, num_sms, stream);
+  });
 }

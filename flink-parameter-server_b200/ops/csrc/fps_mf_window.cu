@@ -19,7 +19,6 @@
 //      together, applies the updates in order, stores each row once and resets every T entry it saw.
 //   3. singleton: a micro-batch that conflicts with itself (an item or a user twice in it) is applied alone
 //      with the per-launch update (pull both rows, red.global.add both deltas): racy as it is today.
-#include <cuda_fp16.h>
 #include <cooperative_groups.h>
 #include "fps_common.cuh"
 #include "fps_mf_args.cuh"
@@ -57,16 +56,18 @@ __device__ __forceinline__ bool win_record(const WinArgs& a, int j, long long i,
                                            float& rating) {
   const unsigned char* base = a.stage + (long long)j * a.slot_bytes;
   if (a.fmt[j] == 1) {
-    const unsigned long long rec = reinterpret_cast<const unsigned long long*>(base)[i];
-    user = (int)(rec >> 38);
-    item = (int)((rec >> 16) & 0x3FFFFFull);
-    rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
+    const FpsRecord<int> rec = fps_record<int>(1, base, nullptr, nullptr, i);
+    user = rec.user;
+    item = rec.item;
+    rating = rec.rating;
     return true;
   }
-  const long long n = a.n[j];
-  user = reinterpret_cast<const int*>(base)[i];
-  item = reinterpret_cast<const int*>(base)[n + i];
-  rating = reinterpret_cast<const float*>(base)[2 * n + i];
+  const long long n = a.n[j];   // arrays: users | items | ratings, n of each
+  const FpsRecord<int> rec =
+      fps_record<int>(0, base, reinterpret_cast<const int*>(base) + n, reinterpret_cast<const float*>(base) + 2 * n, i);
+  user = rec.user;
+  item = rec.item;
+  rating = rec.rating;
   return user >= 0;   // record voided upstream
 }
 

@@ -18,7 +18,6 @@
 //
 // Draws are keyed (position, negative, try, step, seed) as in K5: the output depends on the seed, the step and
 // the stream, never on the grid.
-#include <cuda_fp16.h>
 #include <cooperative_groups.h>
 #include <limits.h>
 #include "fps_common.cuh"
@@ -61,25 +60,8 @@ struct NegDomainArgs {
 };
 
 template <typename IdT>
-__device__ __forceinline__ void ns_record(const NegDomainArgs& a, long long pos, long long& user, long long& item,
-                                          float& rating) {
-  if (a.format == 1) {
-    const unsigned long long rec = reinterpret_cast<const unsigned long long*>(a.users)[pos];
-    user = (long long)(rec >> 38);
-    item = (long long)((rec >> 16) & 0x3FFFFFull);
-    rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
-  } else {
-    user = (long long)reinterpret_cast<const IdT*>(a.users)[pos];
-    item = (long long)reinterpret_cast<const IdT*>(a.items)[pos];
-    rating = a.ratings[pos];
-  }
-}
-
-template <typename IdT>
 __device__ __forceinline__ long long ns_item(const NegDomainArgs& a, long long pos) {
-  if (a.format == 1)
-    return (long long)((reinterpret_cast<const unsigned long long*>(a.users)[pos] >> 16) & 0x3FFFFFull);
-  return (long long)reinterpret_cast<const IdT*>(a.items)[pos];
+  return fps_record_item<IdT>(a.format, a.users, a.items, pos);
 }
 
 // Two 64-bit hashes of try t (and t + 1) of negative j of record pos.
@@ -167,9 +149,9 @@ __global__ void __launch_bounds__(NS_THREADS) fps_neg_seen_kernel(const NegDomai
   // 4. one warp per record: append the positive to the user's ring, then draw from D_p
   const int per = 1 + a.neg_rate;
   for (long long pos = lo + wid; pos < hi; pos += NS_THREADS / 32) {
-    long long user, item;
-    float rating;
-    ns_record<IdT>(a, pos, user, item, rating);
+    const FpsRecord<long long> rec = fps_record<IdT, long long>(a.format, a.users, a.items, a.ratings, pos);
+    const long long user = rec.user, item = rec.item;
+    const float rating = rec.rating;
     const long long dom = (long long)base + (a.scratch[pos] >> 1);
     int mine[NS_MAX_PER_LANE];
     int ring_len = 0;
@@ -303,9 +285,9 @@ __global__ void __launch_bounds__(NS_THREADS) fps_neg_noise_kernel(const NegDoma
        o += (long long)gridDim.x * blockDim.x) {
     const long long pos = o / per;
     const int j = (int)(o - pos * per);
-    long long user, item;
-    float rating;
-    ns_record<IdT>(a, pos, user, item, rating);
+    const FpsRecord<long long> rec = fps_record<IdT, long long>(a.format, a.users, a.items, a.ratings, pos);
+    const long long user = rec.user, item = rec.item;
+    const float rating = rec.rating;
     if (j == 0) {
       a.out_users[o] = (int)user;
       a.out_items[o] = (int)item;

@@ -12,7 +12,6 @@
 //
 // Output: expanded arrays [n_pos * (1 + neg_rate)], record p*(1+neg)+0 = the positive rating and
 // +1.. = its negatives, directly consumable by fps_mf_sgd_fused (neg_rate = 0).
-#include <cuda_fp16.h>
 #include "fps_common.cuh"
 
 #define NEG_MAX_PER_LANE 8  // memory <= 256
@@ -45,18 +44,9 @@ __global__ void __launch_bounds__(256) fps_neg_sample_kernel(const NegArgs a) {
   const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
   const int per = 1 + a.neg_rate;
   for (long long pos = warp; pos < a.n_pos; pos += n_warps) {
-    long long user, item;
-    float rating;
-    if (a.format == 1) {
-      const unsigned long long rec = reinterpret_cast<const unsigned long long*>(a.users)[pos];
-      user = (long long)(rec >> 38);
-      item = (long long)((rec >> 16) & 0x3FFFFFull);
-      rating = __half2float(__ushort_as_half((unsigned short)(rec & 0xFFFFull)));
-    } else {
-      user = (long long)reinterpret_cast<const IdT*>(a.users)[pos];
-      item = (long long)reinterpret_cast<const IdT*>(a.items)[pos];
-      rating = a.ratings[pos];
-    }
+    const FpsRecord<long long> rec = fps_record<IdT, long long>(a.format, a.users, a.items, a.ratings, pos);
+    const long long user = rec.user, item = rec.item;
+    const float rating = rec.rating;
     const long long slot = user / a.user_div;
     int* ring = a.seen + slot * a.memory;
     // append the positive item (ring cursor is bumped atomically: the same user may occur more

@@ -28,6 +28,7 @@
 #include <cooperative_groups.h>
 #include <limits.h>
 #include "fps_common.cuh"
+#include "fps_launch.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -501,15 +502,8 @@ template <int LPR, int VPL, int MINB, int TB>
 static int launch_w2v(const W2vArgs& a, bool cbow, int num_sms, cudaStream_t stream) {
   void (*kern)(const W2vArgs) = cbow ? fps_w2v_cbow_kernel<LPR, VPL, MINB, TB>
                                      : fps_w2v_window_kernel<LPR, VPL, MINB, TB>;
-  int occ = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, W2V_THREADS, 0);
-  if (occ < 1) occ = 1;
-  long long blocks = (long long)num_sms * occ - a.reserve_total;
-  if (blocks < num_sms) blocks = num_sms;
-  const long long groups_per_block = W2V_THREADS / LPR;
-  long long need = (a.n_tokens + groups_per_block - 1) / groups_per_block;   // n_comp <= n_tokens
-  if (need < 1) need = 1;
-  if (blocks > need) blocks = need;
+  const long long blocks = fps_row_grid(kern, W2V_THREADS, W2V_THREADS / LPR, num_sms, a.reserve_total, 0, 1,
+                                        a.n_tokens, 1);   // n_comp <= n_tokens
   kern<<<(int)blocks, W2V_THREADS, 0, stream>>>(a);
   return (int)cudaGetLastError();
 }

@@ -46,7 +46,7 @@ class ShardTableC(C.Structure):
 
 
 class MfArgsC(C.Structure):
-    """Mirror of ``struct MfArgs`` (csrc/fps_core.cu)."""
+    """Mirror of ``struct MfArgs`` (csrc/fps_mf_args.cuh)."""
 
     _fields_ = [
         ("users", C.c_void_p),
@@ -78,7 +78,7 @@ class MfArgsC(C.Structure):
         ("out_staged", C.c_void_p),
         ("out_cap", C.c_longlong),
         ("out_every", C.c_int),
-        ("pad3_", C.c_int),
+        ("reserve_total", C.c_int),
         ("credits", C.c_void_p),
         ("item_acc", ShardTableC),
         ("user_acc_tab", ShardTableC),
@@ -242,18 +242,47 @@ def init_rows(rows: torch.Tensor, dim: int, shard: int, num_shards: int, mode: i
 MF_ERR_MODES = (0, 1, 2)   # the error rules of the pointwise step (fps_mf_args.cuh fps_mf_grad)
 
 
-def _check_pointwise(users, items, ratings, err_mode) -> None:
-    """Refusals shared by :func:`mf_sgd_fused` and :func:`mf_sgd_fused_f64` that need no device tensor."""
-    if int(err_mode) not in MF_ERR_MODES:
-        raise ValueError(f"err_mode must be one of {MF_ERR_MODES}, got {err_mode!r}")
+def _records(users, items, ratings):
+    """Validate a batch of training records and return ``(packed, id_bytes)``.  ``items=None``: ``users`` holds
+    packed64 records (:func:`pack_ratings`; the kernels decode their ids as int32).  Otherwise ``users``, ``items``
+    and ``ratings`` are arrays of one length, with one int32 or int64 id dtype and float32 ratings.  The dtype and
+    length refusals come before the CUDA checks."""
     if items is None:
         if users.dtype != torch.int64:
             raise TypeError("packed rating records must be an int64 tensor (see pack_ratings)")
-        return
+        _req(users, "users")
+        return True, 4
     if users.dtype != items.dtype:
         raise TypeError("users and items must share an integer dtype")
+    id_bytes = _id_bytes(users)
+    if ratings.dtype != torch.float32:
+        raise TypeError(f"ratings must be {torch.float32}, got {ratings.dtype}")
     if items.numel() != users.numel() or ratings.numel() != users.numel():
         raise ValueError("users, items and ratings must have the same length")
+    _req(users, "users"); _req(items, "items"); _req(ratings, "ratings")
+    return False, id_bytes
+
+
+def _check_err_mode(err_mode) -> None:
+    if int(err_mode) not in MF_ERR_MODES:
+        raise ValueError(f"err_mode must be one of {MF_ERR_MODES}, got {err_mode!r}")
+
+
+def _set_row_acc(a, name: str, acc, table, sharded: bool) -> None:
+    """Row-wise AdaGrad accumulators of the ``name`` rows (``user`` / ``anchor``) of ``a``: a stride-1
+    :class:`ShardTableC` in ``<name>_acc_tab`` when the row table is sharded, else a float32 tensor with one entry
+    per row of ``table`` in ``<name>_acc``."""
+    if sharded:
+        if not isinstance(acc, ShardTableC) or int(acc.stride) != 1:
+            raise ValueError(f"a sharded {name} table needs a stride-1 ShardTableC {name}_acc")
+        setattr(a, f"{name}_acc_tab", acc)
+        return
+    if not torch.is_tensor(acc):
+        raise ValueError(f"a worker-local {name} table needs a float32 {name}_acc tensor")
+    _req(acc, f"{name}_acc", torch.float32)
+    if acc.numel() < table.shape[0]:
+        raise ValueError(f"{name}_acc must hold one accumulator per {name} row")
+    setattr(a, f"{name}_acc", acc.data_ptr())
 
 
 def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor,
@@ -262,7 +291,7 @@ def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
                  step: int = 0, stats: Optional[torch.Tensor] = None,
                  nan_flag: Optional[torch.Tensor] = None, max_inflight_rows: int = 0,
                  kernel: Optional[str] = None, push_tab: Optional[ShardTableC] = None,
-                 l2_hints: bool = False, reserve_ctas: int = 0, reserve_total: int = 0,
+                 l2_hints: bool = False, reserve_total: int = 0,
                  progress: Optional[torch.Tensor] = None, output=None,
                  credits: Optional[torch.Tensor] = None, item_acc: Optional[ShardTableC] = None,
                  user_acc=None) -> None:
@@ -280,17 +309,15 @@ def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
 
     ``err_mode``: 0 ``e = sigmoid(r - u.v)``, 1 ``e = r - u.v``, 2 ``e = r - sigmoid(u.v)``.  ``neg_rate > 0``
     draws that many negatives per record in the kernel, uniform over ``[0, num_items)`` and never the
-    positive, so it needs ``num_items >= 2``."""
-    _check_pointwise(users, items, ratings, err_mode)
+    positive, so it needs ``num_items >= 2``.  ``reserve_total``: CTA slots the grid leaves free for a kernel running
+    next to it (the replica exchange)."""
+    _check_err_mode(err_mode)
     if int(neg_rate) > 0 and int(num_items) < 2:
         raise ValueError(f"sampled negatives need num_items >= 2, got {num_items}")
-    _req(users, "users")
+    packed, id_bytes = _records(users, items, ratings)
     user_sharded = isinstance(user_table, ShardTableC)
     if not user_sharded:
         _req(user_table, "user_table", torch.float32)
-    packed = items is None
-    if not packed:
-        _req(items, "items"); _req(ratings, "ratings", torch.float32)
     if (user_table.stride if user_sharded else user_table.shape[1]) != item_tab.stride:
         raise ValueError("user table stride must equal item table stride")
     a = MfArgsC()
@@ -330,33 +357,22 @@ def mf_sgd_fused(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
         if int(item_acc.stride) != 1:
             raise ValueError("item_acc must be a stride-1 accumulator table")
         a.item_acc = item_acc
-        if user_sharded:
-            if not isinstance(user_acc, ShardTableC) or int(user_acc.stride) != 1:
-                raise ValueError("a sharded user table needs a stride-1 ShardTableC user_acc")
-            a.user_acc_tab = user_acc
-        else:
-            if not torch.is_tensor(user_acc):
-                raise ValueError("a worker-local user table needs a float32 user_acc tensor")
-            _req(user_acc, "user_acc", torch.float32)
-            if user_acc.numel() < user_table.shape[0]:
-                raise ValueError("user_acc must hold one accumulator per user row")
-            a.user_acc = user_acc.data_ptr()
+        _set_row_acc(a, "user", user_acc, user_table, user_sharded)
         variant = "reg"
     elif user_acc is not None:
         raise ValueError("user_acc needs item_acc")
-    lib().fps_set_mf_reserve(int(reserve_ctas))
-    lib().fps_set_mf_reserve_total(int(reserve_total))
+    a.reserve_total = max(0, int(reserve_total))
     rv = os.environ.get("FPS_MF_REG_VARIANT")
     if rv is not None:
         lib().fps_set_mf_reg_variant(int(rv))
     if variant == "tma":
-        code = lib().fps_mf_sgd_tma(C.byref(a), _id_bytes(users), int(max_inflight_rows),
+        code = lib().fps_mf_sgd_tma(C.byref(a), id_bytes, int(max_inflight_rows),
                                     sm_count(users.device.index), _stream())
         if code != -1002:  # -1002: rows too large for the smem ring -> register-staged kernel
             _check(code, "mf_sgd_tma")
             _bump()
             return
-    _check(lib().fps_mf_sgd_fused(C.byref(a), 4 if packed else _id_bytes(users), int(max_inflight_rows),
+    _check(lib().fps_mf_sgd_fused(C.byref(a), id_bytes, int(max_inflight_rows),
                                   sm_count(users.device.index), _stream()), "mf_sgd_fused")
     _bump()
 
@@ -452,21 +468,10 @@ class BprArgsC(C.Structure):
 
 def _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, negatives, n_neg, num_items, seed,
                    step, anchor_div, cand_div, stats, n_stats, nan_flag, push_tab, reserve_total):
-    """The validated :class:`BprArgsC` of :func:`mf_bpr_fused` / :func:`mf_warp_fused`, and whether ``users`` holds
-    packed64 records."""
-    _req(users, "users")
-    packed = items is None
-    if packed:
-        if users.dtype != torch.int64:
-            raise TypeError("packed rating records must be an int64 tensor (see pack_ratings)")
-        id_dtype = torch.int32
-    else:
-        _req(items, "items"); _req(ratings, "ratings", torch.float32)
-        if users.dtype != items.dtype:
-            raise TypeError("users and items must share an integer dtype")
-        if items.numel() != users.numel() or ratings.numel() != users.numel():
-            raise ValueError("users, items and ratings must have the same length")
-        id_dtype = users.dtype
+    """The validated :class:`BprArgsC` of :func:`mf_bpr_fused` / :func:`mf_warp_fused`, and the id width of the
+    records (:func:`_records`)."""
+    packed, id_bytes = _records(users, items, ratings)
+    id_dtype = torch.int32 if id_bytes == 4 else torch.int64
     n_pos = users.numel()
     a = BprArgsC()
     strides = []
@@ -514,7 +519,7 @@ def _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, neg
     a.n_pos = n_pos; a.num_items = int(max(num_items, 1))
     a.seed = seed & (2**64 - 1); a.step = int(step)
     a.lr = float(lr); a.reg = float(reg); a.reserve_total = int(reserve_total)
-    return a, packed
+    return a, id_bytes
 
 
 def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Optional[torch.Tensor],
@@ -543,28 +548,18 @@ def mf_bpr_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Op
     :class:`ShardTableC` of candidate accumulators (``cand_table`` must then be a ShardTableC, without
     ``push_tab``); ``anchor_acc`` a float32 ``[rows]`` tensor, or a stride-1 ShardTableC when ``anchor_table``
     is one."""
-    a, packed = _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, negatives, n_neg, num_items,
-                               seed, step, anchor_div, cand_div, stats, 3, nan_flag, push_tab, reserve_total)
+    a, id_bytes = _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, negatives, n_neg, num_items,
+                                 seed, step, anchor_div, cand_div, stats, 3, nan_flag, push_tab, reserve_total)
     if cand_acc is not None:
         if not a.cand_sharded or push_tab is not None:
             raise ValueError("row-wise AdaGrad needs a ShardTableC cand_table and no push_tab")
         if int(cand_acc.stride) != 1:
             raise ValueError("cand_acc must be a stride-1 accumulator table")
         a.cand_acc = cand_acc
-        if a.anchor_sharded:
-            if not isinstance(anchor_acc, ShardTableC) or int(anchor_acc.stride) != 1:
-                raise ValueError("a sharded anchor table needs a stride-1 ShardTableC anchor_acc")
-            a.anchor_acc_tab = anchor_acc
-        else:
-            if not torch.is_tensor(anchor_acc):
-                raise ValueError("a worker-local anchor table needs a float32 anchor_acc tensor")
-            _req(anchor_acc, "anchor_acc", torch.float32)
-            if anchor_acc.numel() < anchor_table.shape[0]:
-                raise ValueError("anchor_acc must hold one accumulator per anchor row")
-            a.anchor_acc = anchor_acc.data_ptr()
+        _set_row_acc(a, "anchor", anchor_acc, anchor_table, bool(a.anchor_sharded))
     elif anchor_acc is not None:
         raise ValueError("anchor_acc needs cand_acc")
-    _check(lib().fps_mf_bpr_fused(C.byref(a), 4 if packed else _id_bytes(users), int(max_inflight_rows),
+    _check(lib().fps_mf_bpr_fused(C.byref(a), id_bytes, int(max_inflight_rows),
                                   sm_count(users.device.index), _stream()), "mf_bpr_fused")
     _bump()
 
@@ -595,11 +590,11 @@ def mf_warp_fused(users: torch.Tensor, items: Optional[torch.Tensor], ratings: O
         raise ValueError(f"margin must be finite, got {margin!r}")
     if int(trial_block) not in (0,) + WARP_TRIAL_BLOCKS:
         raise ValueError(f"trial_block must be 0 or one of {WARP_TRIAL_BLOCKS}, got {trial_block!r}")
-    a, packed = _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, negatives, n_neg, num_items,
-                               seed, step, anchor_div, cand_div, stats, 4, nan_flag, push_tab, reserve_total)
+    a, id_bytes = _pairwise_args(users, items, ratings, anchor_table, cand_table, lr, reg, negatives, n_neg, num_items,
+                                 seed, step, anchor_div, cand_div, stats, 4, nan_flag, push_tab, reserve_total)
     a.margin = float(margin)
     a.rank_items = int(rank_items) if int(rank_items) > 0 else int(a.num_items)
-    _check(lib().fps_mf_warp_fused(C.byref(a), 4 if packed else _id_bytes(users), int(trial_block),
+    _check(lib().fps_mf_warp_fused(C.byref(a), id_bytes, int(trial_block),
                                    int(max_inflight_rows), sm_count(users.device.index), _stream()), "mf_warp_fused")
     _bump()
 
@@ -622,11 +617,9 @@ def mf_sgd_fused_f64(users: torch.Tensor, items: Optional[torch.Tensor], ratings
     """fp64 fused pull + SGD + push (csrc/fps_mf_f64.cu): ``user_table`` is float64 ``[n, k_pad]``, the shards
     of ``item_tab`` hold doubles (stride counted in 4-byte cells).  ``items=None``: packed64 records.
     ``err_mode`` as for :func:`mf_sgd_fused`."""
-    _check_pointwise(users, items, ratings, err_mode)
-    _req(users, "users"); _req(user_table, "user_table", torch.float64)
-    packed = items is None
-    if not packed:
-        _req(items, "items"); _req(ratings, "ratings", torch.float32)
+    _check_err_mode(err_mode)
+    packed, id_bytes = _records(users, items, ratings)
+    _req(user_table, "user_table", torch.float64)
     if user_table.shape[1] * 2 != item_tab.stride:
         raise ValueError("user table width must equal the item row width")
     a = MfArgsC()
@@ -640,7 +633,7 @@ def mf_sgd_fused_f64(users: torch.Tensor, items: Optional[torch.Tensor], ratings
     a.stats = stats.data_ptr() if stats is not None else None
     a.nan_flag = nan_flag.data_ptr() if nan_flag is not None else None
     a.item_tab = item_tab
-    _check(lib().fps_mf_sgd_fused_f64(C.byref(a), 4 if packed else _id_bytes(users),
+    _check(lib().fps_mf_sgd_fused_f64(C.byref(a), id_bytes,
                                       sm_count(users.device.index), _stream()), "mf_sgd_fused_f64")
     _bump()
 
@@ -666,10 +659,8 @@ def neg_sample(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Opti
     place).  Returns ``(users, items, ratings)`` int32/int32/float32 of length ``n*(1+neg_rate)``;
     a negative that could not be found in ``max_tries`` draws has user == -1 (skipped downstream).
     ``items=None``: ``users`` holds packed64 records."""
-    _req(users, "users"); _req(seen, "seen", torch.int32); _req(seen_pos, "seen_pos", torch.int32)
-    packed = items is None
-    if not packed:
-        _req(items, "items"); _req(ratings, "ratings", torch.float32)
+    packed, id_bytes = _records(users, items, ratings)
+    _req(seen, "seen", torch.int32); _req(seen_pos, "seen_pos", torch.int32)
     n = users.numel()
     per = 1 + int(neg_rate)
     dev = users.device
@@ -685,7 +676,7 @@ def neg_sample(users: torch.Tensor, items: Optional[torch.Tensor], ratings: Opti
     a.seen = seen.data_ptr(); a.seen_pos = seen_pos.data_ptr(); a.memory = int(seen.shape[1])
     a.user_div = int(user_div); a.max_tries = int(max_tries)
     a.out_users = ou.data_ptr(); a.out_items = oi.data_ptr(); a.out_ratings = orat.data_ptr()
-    _check(lib().fps_neg_sample(C.byref(a), 4 if packed else _id_bytes(users),
+    _check(lib().fps_neg_sample(C.byref(a), id_bytes,
                                 sm_count(dev.index), _stream()), "neg_sample")
     _bump()
     return ou, oi, orat
@@ -707,17 +698,7 @@ class NegDomainArgsC(C.Structure):
 
 
 def _neg_domain_args(users, items, ratings, neg_rate: int, seed: int, step: int, max_tries: int):
-    _req(users, "users")
-    packed = items is None
-    if packed:
-        if users.dtype != torch.int64:
-            raise TypeError("packed rating records must be an int64 tensor (see pack_ratings)")
-    else:
-        _req(items, "items"); _req(ratings, "ratings", torch.float32)
-        if users.dtype != items.dtype:
-            raise TypeError("users and items must share an integer dtype")
-        if items.numel() != users.numel() or ratings.numel() != users.numel():
-            raise ValueError("users, items and ratings must have the same length")
+    packed, id_bytes = _records(users, items, ratings)
     if int(neg_rate) < 0:
         raise ValueError("neg_rate must be >= 0")
     n, per, dev = users.numel(), 1 + int(neg_rate), users.device
@@ -730,7 +711,7 @@ def _neg_domain_args(users, items, ratings, neg_rate: int, seed: int, step: int,
     a.n_pos = n; a.neg_rate = int(neg_rate); a.format = 1 if packed else 0
     a.seed = seed & (2**64 - 1); a.step = int(step); a.max_tries = int(max_tries)
     a.out_users, a.out_items, a.out_ratings = (t.data_ptr() for t in out)
-    return a, out, (4 if packed else _id_bytes(users))
+    return a, out, id_bytes
 
 
 def seen_registry(num_items: int, device) -> tuple:
@@ -981,23 +962,18 @@ def bucket_by_item(users: torch.Tensor, items: Optional[torch.Tensor], ratings: 
     ``2 * BUCKET_MAX`` elements.  ``pending``: optional int64 ``[num_shards]`` device counters that
     receive the number of records per destination shard (feed of the device-side flush policy).
     Returns the reordered ``(users, items, ratings)`` (new tensors)."""
-    _req(users, "users"); _req(scratch, "scratch", torch.int32)
-    packed = items is None
+    packed, id_bytes = _records(users, items, ratings)
+    _req(scratch, "scratch", torch.int32)
     a = BucketArgsC()
     a.users = users.data_ptr(); a.n = users.numel()
     ou = torch.empty_like(users)
     oi = orat = None
     a.out_users = ou.data_ptr()
-    if packed:
-        if users.dtype != torch.int64:
-            raise TypeError("packed rating records must be an int64 tensor")
-        a.format = 1; a.id_bytes = 8
-    else:
-        _req(items, "items"); _req(ratings, "ratings", torch.float32)
+    a.format = 1 if packed else 0; a.id_bytes = id_bytes
+    if not packed:
         oi, orat = torch.empty_like(items), torch.empty_like(ratings)
         a.items = items.data_ptr(); a.ratings = ratings.data_ptr()
         a.out_items = oi.data_ptr(); a.out_ratings = orat.data_ptr()
-        a.format = 0; a.id_bytes = _id_bytes(users)
     a.shift = int(shift); a.n_buckets = int(n_buckets); a.scratch = scratch.data_ptr()
     a.num_shards = max(1, int(num_shards)); a.shard_shift = log2_or_neg(a.num_shards)
     a.rps = int(rows_per_shard)
@@ -1010,6 +986,8 @@ def bucket_by_item(users: torch.Tensor, items: Optional[torch.Tensor], ratings: 
 
 
 PACK_USER_BITS, PACK_ITEM_BITS = 26, 22
+PACK_ITEM_SHIFT = 16                                 # below it: the fp16 rating
+PACK_USER_SHIFT = PACK_ITEM_SHIFT + PACK_ITEM_BITS   # 38 (csrc/fps_common.cuh FPS_REC_*)
 
 
 def pack_ratings(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor) -> torch.Tensor:
@@ -1018,7 +996,7 @@ def pack_ratings(users: torch.Tensor, items: torch.Tensor, ratings: torch.Tensor
     if int(users.max()) >= 1 << PACK_USER_BITS or int(items.max()) >= 1 << PACK_ITEM_BITS:
         raise ValueError("ids exceed the packed64 record range (user < 2^26, item < 2^22)")
     r16 = ratings.to(torch.float16).view(torch.int16).to(torch.int64) & 0xFFFF
-    return (users.to(torch.int64) << 38) | (items.to(torch.int64) << 16) | r16
+    return (users.to(torch.int64) << PACK_USER_SHIFT) | (items.to(torch.int64) << PACK_ITEM_SHIFT) | r16
 
 
 def pull_gather(tab: ShardTableC, ids: torch.Tensor, out: torch.Tensor, touch: bool = False,
