@@ -123,6 +123,7 @@ __global__ void __launch_bounds__(BK_THREADS) fps_bucket_deal_kernel(const Bucke
 }
 
 extern "C" int fps_bucket_by_item(const BucketArgs* a, int num_sms, cudaStream_t stream) {
+  if (a->num_shards < 1 || a->num_shards > FPS_MAX_SHARDS) return -1302;   // ohist has FPS_MAX_SHARDS entries
   if (a->n <= 0) return 0;
   if (a->n_buckets < 1 || a->n_buckets > BK_MAX || a->n >= (1ll << 32)) return -1301;
   int occ = 0;

@@ -68,6 +68,9 @@ extern "C" const char* fps_error_string(int code) {
   if (code == -1000) return "dim too large for fused kernel";
   if (code == -1001) return "unsupported id width";
   if (code == -1009) return "row-wise AdaGrad does not support this kernel variant";
+  if (code == -1302 || code == -1403) return "num_shards outside [1, 16]";
+  if (code == -1404) return "row stride is not a positive multiple of 4 floats";
+  if (code == -1405) return "slot range outside [0, rows_per_shard]";
   if (code < 0) return "fps: invalid argument";
   return cudaGetErrorString((cudaError_t)code);
 }

@@ -109,6 +109,22 @@ __device__ __forceinline__ int ex_nth_set_bit(unsigned mask, int n) {
   return __ffs(mask) - 1;
 }
 
+// Slots [lo, hi) of destination o in one launch, the same in both exchange kernels: the whole
+// [slot_lo, slot_hi), or when sliced one `slice_len` slice of it, slice = (flushes[o] + o + slice_offset) %
+// slices (flushes[o] was bumped by the policy kernel).  Slices past slot_hi are empty (lo == hi).
+__device__ __forceinline__ void ex_dest_range(const ExchArgs& a, int o, bool sliced, long long slice_len,
+                                              long long& lo, long long& hi) {
+  lo = a.slot_lo;
+  hi = a.slot_hi;
+  if (sliced) {
+    const long long sl = (long long)((a.state->flushes[o] + (unsigned long long)(o + a.slice_offset)) %
+                                     (unsigned long long)a.slices);
+    lo = a.slot_lo + sl * slice_len;
+    hi = lo + slice_len < a.slot_hi ? lo + slice_len : a.slot_hi;
+    if (lo > hi) lo = hi;
+  }
+}
+
 __global__ void __launch_bounds__(EX_THREADS, 1)
     fps_replica_exchange_kernel(const __grid_constant__ ExchArgs a) {
   extern __shared__ __align__(128) unsigned char ex_smem[];
@@ -141,14 +157,8 @@ __global__ void __launch_bounds__(EX_THREADS, 1)
   }
   if (threadIdx.x < a.master.num_shards) {
     const int o = threadIdx.x;
-    long long lo = a.slot_lo, hi = a.slot_hi;
-    if (sliced) {   // the rotating sub-range of this destination (flushes[o] was bumped by the policy kernel)
-      const long long sl = (long long)((a.state->flushes[o] + (unsigned long long)(o + a.slice_offset)) %
-                                       (unsigned long long)a.slices);
-      lo = a.slot_lo + sl * slice_len;
-      hi = lo + slice_len < a.slot_hi ? lo + slice_len : a.slot_hi;
-      if (lo > hi) lo = hi;
-    }
+    long long lo, hi;
+    ex_dest_range(a, o, sliced, slice_len, lo, hi);
     seg_lo[o] = lo;
     seg_hi[o] = hi;
   }
@@ -251,12 +261,16 @@ __global__ void __launch_bounds__(256)
   unsigned mask = (a.state != nullptr ? a.state->mask : a.mask_override) & ~a.skip_mask;
   const int stride = a.master.stride;
   const int nvec = stride >> 2;
-  const long long n_slots = a.slot_hi - a.slot_lo;
-  const long long per_seg = n_slots * nvec;
+  const bool sliced = a.slices > 1 && a.state != nullptr;
+  const long long seg_slots = a.slot_hi - a.slot_lo;
+  const long long slice_len = sliced ? (seg_slots + a.slices - 1) / a.slices : seg_slots;
   for (int o = 0; o < a.master.num_shards; ++o) {
     if (!((mask >> o) & 1u)) continue;
-    float* m = a.master.base[o] + (size_t)a.slot_lo * stride;
-    const size_t seg_off = ((size_t)o * (size_t)a.rps + (size_t)a.slot_lo) * (size_t)stride;
+    long long lo, hi;
+    ex_dest_range(a, o, sliced, slice_len, lo, hi);
+    const long long per_seg = (hi - lo) * nvec;
+    float* m = a.master.base[o] + (size_t)lo * stride;
+    const size_t seg_off = ((size_t)o * (size_t)a.rps + (size_t)lo) * (size_t)stride;
     float* cseg = a.cache + seg_off;
     float* bseg = a.base + seg_off;
     for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < per_seg;
@@ -277,9 +291,15 @@ __global__ void __launch_bounds__(256)
 }
 
 // n_ctas: CTAs of the exchange grid (the training kernel leaves that many CTA slots free);
-// n_stages <= 0 picks the default ring depth.  Returns 0 or an error code.
+// n_stages <= 0 picks the default ring depth (4), more than EX_MAX_STAGES is clamped to it.  Refuses a shard
+// count outside [1, FPS_MAX_SHARDS] (the kernels index per-shard arrays of that size), a stride that is not a
+// positive multiple of 4 (16-byte bulk copies and vector reductions) and a slot range outside [0, rps).
+// An empty range (slot_hi <= slot_lo) launches nothing.  Returns 0 or an error code.
 extern "C" int fps_replica_exchange(const ExchArgs* args, int n_ctas, cudaStream_t stream) {
   ExchArgs a = *args;
+  if (a.master.num_shards < 1 || a.master.num_shards > FPS_MAX_SHARDS) return -1403;
+  if (a.master.stride < 4 || a.master.stride % 4 != 0) return -1404;
+  if (a.slot_lo < 0 || a.slot_hi > a.rps) return -1405;
   if (a.slot_hi <= a.slot_lo) return 0;
   if (n_ctas < 1) n_ctas = 1;
   const int nvec = a.master.stride >> 2;

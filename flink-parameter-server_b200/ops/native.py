@@ -263,6 +263,12 @@ def _records(users, items, ratings):
     return False, id_bytes
 
 
+def _shard_count(num_shards) -> None:
+    """The device kernels keep per-shard state in arrays of ``FPS_MAX_SHARDS`` entries."""
+    if not 1 <= int(num_shards) <= FPS_MAX_SHARDS:
+        raise ValueError(f"num_shards must be in [1, {FPS_MAX_SHARDS}], got {num_shards}")
+
+
 def _check_err_mode(err_mode) -> None:
     if int(err_mode) not in MF_ERR_MODES:
         raise ValueError(f"err_mode must be one of {MF_ERR_MODES}, got {err_mode!r}")
@@ -961,7 +967,9 @@ def bucket_by_item(users: torch.Tensor, items: Optional[torch.Tensor], ratings: 
     ``items=None``: ``users`` holds packed64 records.  ``scratch``: int32 device tensor of
     ``2 * BUCKET_MAX`` elements.  ``pending``: optional int64 ``[num_shards]`` device counters that
     receive the number of records per destination shard (feed of the device-side flush policy).
-    Returns the reordered ``(users, items, ratings)`` (new tensors)."""
+    Returns the reordered ``(users, items, ratings)`` (new tensors).  ``num_shards`` outside
+    ``[1, FPS_MAX_SHARDS]`` is refused before any CUDA check."""
+    _shard_count(num_shards)
     packed, id_bytes = _records(users, items, ratings)
     _req(scratch, "scratch", torch.int32)
     a = BucketArgsC()
@@ -975,7 +983,7 @@ def bucket_by_item(users: torch.Tensor, items: Optional[torch.Tensor], ratings: 
         a.items = items.data_ptr(); a.ratings = ratings.data_ptr()
         a.out_items = oi.data_ptr(); a.out_ratings = orat.data_ptr()
     a.shift = int(shift); a.n_buckets = int(n_buckets); a.scratch = scratch.data_ptr()
-    a.num_shards = max(1, int(num_shards)); a.shard_shift = log2_or_neg(a.num_shards)
+    a.num_shards = int(num_shards); a.shard_shift = log2_or_neg(a.num_shards)
     a.rps = int(rows_per_shard)
     if pending is not None:
         _req(pending, "pending", torch.int64)
@@ -1157,9 +1165,13 @@ def flush_policy(state: torch.Tensor, num_dest: int, count_max: int = 0, interva
     """Device-side CountLogic / TimerLogic (CountLogic.scala:5-29, TimerLogic.scala:6-51) for the
     per-destination send buffers of a replica: decides ON THE GPU which destinations to flush now
     (messages buffered >= ``count_max`` and/or ``globaltimer`` deadline ``interval_ns`` passed, OR /
-    AND) and leaves the bit mask in ``state`` (int64 ``[FLUSH_STATE_WORDS]``) for the exchange kernel."""
+    AND) and leaves the bit mask in ``state`` (int64 ``[FLUSH_STATE_WORDS]``) for the exchange kernel.
+    ``num_dest`` outside ``[1, FPS_MAX_SHARDS]`` and a short ``state`` are refused before any CUDA check."""
+    if not 1 <= int(num_dest) <= FPS_MAX_SHARDS:
+        raise ValueError(f"num_dest must be in [1, {FPS_MAX_SHARDS}], got {num_dest}")
+    if state.numel() < FLUSH_STATE_WORDS:
+        raise ValueError(f"state must hold {FLUSH_STATE_WORDS} int64 words, got {state.numel()}")
     _req(state, "state", torch.int64)
-    assert state.numel() >= FLUSH_STATE_WORDS
     p = FlushPolicyC()
     p.count_max = int(count_max); p.interval_ns = int(interval_ns); p.add_uniform = int(add_uniform)
     p.require_all = int(bool(require_all)); p.force = int(bool(force)); p.num_dest = int(num_dest)
@@ -1185,14 +1197,27 @@ def replica_exchange(master: ShardTableC, cache: torch.Tensor, base: torch.Tenso
     """One delta exchange between an owner-major replica and its master shards for the destinations
     flagged in ``state`` (written by :func:`flush_policy`) or in ``mask``: push ``replica - base``
     (REDG over NVLink), fold ``master - base`` into the replica, ``base <- master + pushed delta``.
-    TMA bulk reads through a shared-memory ring; ``n_ctas`` CTAs.  csrc/fps_replica.cu."""
-    _req(cache, "cache", torch.float32); _req(base, "base", torch.float32)
+    TMA bulk reads through a shared-memory ring; ``n_ctas`` CTAs.  csrc/fps_replica.cu.
+
+    Each flagged destination moves its slots ``[slot_lo, slot_hi)``; with ``state`` and ``slices > 1``, one
+    ``ceil((slot_hi - slot_lo) / slices)``-slot slice of them, slice ``(flushes[o] + o + slice_offset) %
+    slices``, in both the TMA kernel and the kernel for rows wider than 2048 floats.  An empty range is a
+    no-op.  ``n_stages <= 0`` means 4, more than 8 means 8.  Refused before any CUDA check: a shard count
+    outside ``[1, FPS_MAX_SHARDS]``, a row stride that is not a positive multiple of 4 floats, and
+    ``slot_lo < 0`` or ``slot_hi > rows_per_shard``."""
+    _shard_count(master.num_shards)
     rps = int(master.rows_per_shard)
+    if master.stride < 4 or master.stride % 4:
+        raise ValueError(f"master stride must be a positive multiple of 4 floats, got {master.stride}")
+    slot_hi = rps if slot_hi is None else int(slot_hi)
+    if int(slot_lo) < 0 or slot_hi > rps:
+        raise ValueError(f"slot range [{slot_lo}, {slot_hi}) is outside [0, {rps}]")
+    _req(cache, "cache", torch.float32); _req(base, "base", torch.float32)
     assert cache.shape == base.shape and cache.shape[1] == master.stride
     assert cache.shape[0] == rps * master.num_shards
     a = ExchArgsC()
     a.master = master; a.cache = cache.data_ptr(); a.base = base.data_ptr(); a.rps = rps
-    a.slot_lo = int(slot_lo); a.slot_hi = rps if slot_hi is None else int(slot_hi)
+    a.slot_lo = int(slot_lo); a.slot_hi = slot_hi
     if state is not None:
         _req(state, "state", torch.int64)
         a.state = state.data_ptr()

@@ -1,6 +1,6 @@
-"""Record-batch refusals of every binding that takes training records, and the ctypes mirrors of the MF argument
-blocks against the C structs.  No GPU: the refusals come before any CUDA check, the layouts are read from a host
-program compiled with nvcc."""
+"""Record-batch refusals of every binding that takes training records, and the ctypes mirrors of the kernel argument
+blocks and the flush state against the C structs.  No GPU: the refusals come before any CUDA check, the layouts
+are read from a host program compiled with nvcc."""
 import ctypes as C
 import shutil
 import subprocess
@@ -65,26 +65,47 @@ def test_ratings_must_be_float32(name):
         BINDINGS[name](u, i, torch.ones(4, dtype=torch.float64))
 
 
-# ---- ctypes mirrors of MfArgs and BprArgs ---------------------------------------------------------------------
+# ---- ctypes mirrors of the argument blocks ---------------------------------------------------------------------
 
 def _nvcc():
     cand = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     return cand if Path(cand).exists() else None
 
 
-@pytest.mark.skipif(_nvcc() is None, reason="nvcc not found")
-@pytest.mark.parametrize("struct, mirror", [("MfArgs", native.MfArgsC), ("BprArgs", native.BprArgsC)])
-def test_args_mirror_matches_the_c_layout(tmp_path, struct, mirror):
-    lines = [f'  printf("sizeof %zu\\n", sizeof({struct}));']
-    lines += [f'  printf("{f} %zu\\n", offsetof({struct}, {f}));' for f, _ in mirror._fields_]
+def _layout(tmp_path, header, lines):
+    """Run a host program that includes ``header`` and prints ``lines`` (``key value`` pairs)."""
     src = tmp_path / "layout.cu"
-    src.write_text('#include <cstddef>\n#include <cstdio>\n#include "fps_mf_args.cuh"\nint main() {\n'
+    src.write_text(f'#include <cstddef>\n#include <cstdio>\n#include "{header}"\nint main() {{\n'
                    + "\n".join(lines) + "\n  return 0;\n}\n")
     exe = tmp_path / "layout"
     subprocess.run([_nvcc(), *build.NVCC_FLAGS, "-I", str(build.CSRC), str(src), "-o", str(exe)], check=True,
                    capture_output=True)
-    got = dict(line.split() for line in subprocess.run([str(exe)], check=True, capture_output=True,
-                                                       text=True).stdout.splitlines())
+    return dict(line.split() for line in subprocess.run([str(exe)], check=True, capture_output=True,
+                                                        text=True).stdout.splitlines())
+
+
+STRUCT_HEADER = {"MfArgs": "fps_mf_args.cuh", "BprArgs": "fps_mf_args.cuh", "ExchArgs": "fps_replica.cu",
+                 "FlushPolicy": "fps_replica.cu", "BucketArgs": "fps_bucket.cu"}   # where each struct lives
+
+
+@pytest.mark.skipif(_nvcc() is None, reason="nvcc not found")
+@pytest.mark.parametrize("struct, mirror", [
+    ("MfArgs", native.MfArgsC), ("BprArgs", native.BprArgsC), ("ExchArgs", native.ExchArgsC),
+    ("FlushPolicy", native.FlushPolicyC), ("BucketArgs", native.BucketArgsC)])
+def test_args_mirror_matches_the_c_layout(tmp_path, struct, mirror):
+    lines = [f'  printf("sizeof %zu\\n", sizeof({struct}));']
+    lines += [f'  printf("{f} %zu\\n", offsetof({struct}, {f}));' for f, _ in mirror._fields_]
     want = {f: str(getattr(mirror, f).offset) for f, _ in mirror._fields_}
     want["sizeof"] = str(C.sizeof(mirror))
-    assert got == want
+    assert _layout(tmp_path, STRUCT_HEADER[struct], lines) == want
+
+
+@pytest.mark.skipif(_nvcc() is None, reason="nvcc not found")
+def test_flush_state_words_match_the_c_layout(tmp_path):
+    fields = {"pending": native.FLUSH_PENDING, "last_ns": native.FLUSH_LAST_NS, "flushes": native.FLUSH_COUNT,
+              "mask": native.FLUSH_MASK}
+    lines = ['  printf("sizeof %zu\\n", sizeof(FlushState));']
+    lines += [f'  printf("{f} %zu\\n", offsetof(FlushState, {f}));' for f in fields]
+    want = {f: str(8 * w) for f, w in fields.items()}
+    want["sizeof"] = str(8 * native.FLUSH_STATE_WORDS)
+    assert _layout(tmp_path, "fps_replica.cu", lines) == want
