@@ -71,6 +71,11 @@ extern "C" const char* fps_error_string(int code) {
   if (code == -1302 || code == -1403) return "num_shards outside [1, 16]";
   if (code == -1404) return "row stride is not a positive multiple of 4 floats";
   if (code == -1405) return "slot range outside [0, rows_per_shard]";
+  if (code == -1601) return "factorization machine: row stride is not a positive multiple of 4 floats";
+  if (code == -1602) return "factorization machine: dim outside [1, stride]";
+  if (code == -1603) return "factorization machine: unknown loss code";
+  if (code == -1604) return "factorization machine: n or nnz out of range";
+  if (code == -1605) return "factorization machine: bias on without its accumulator";
   if (code < 0) return "fps: invalid argument";
   return cudaGetErrorString((cudaError_t)code);
 }

@@ -92,3 +92,34 @@ def topic_corpus(vocab: int, topics: int, sentence_len: int, sentences: int, see
         r = torch.multinomial(w, rows.numel() * sentence_len, replacement=True, generator=g)
         out[rows, :sentence_len] = (r * topics + k).view(rows.numel(), sentence_len)
     return out.reshape(-1)
+
+
+def planted_fm(num_features: int, fields: int, k: int, n: int, seed: int = 0, loss: str = "logistic"):
+    """One-hot examples with labels from a planted factorization machine, for the FM quality gates.
+
+    Field ``f`` owns the ids ``[f * per, (f + 1) * per)``, ``per = num_features // fields``; every example takes one
+    id per field, uniformly.  The planted model has ``w*_i = U(-1, 1)`` and ``v*_i,f = U(-1, 1)`` hashed from
+    ``(id, f, seed)``; its score is the linear term scaled to unit standard deviation plus the pairwise term
+    ``sum_{a<b} <v*_a, v*_b>`` scaled to standard deviation 2, so a model with factors can beat a linear one.
+    ``"logistic"``: ``y ~ Bernoulli(sigmoid(score))``; ``"squared"``: ``y = score + N(0, 0.25)``.
+
+    Returns ``(row_ptr, cols, labels)`` on the CPU: int64 ``[n + 1]``, int64 ``[n * fields]``, float32 ``[n]``."""
+    if fields < 1 or num_features < fields or k < 1 or n < 0:
+        raise ValueError("planted_fm needs fields >= 1, num_features >= fields, k >= 1 and n >= 0")
+    if loss not in ("logistic", "squared"):
+        raise ValueError(f"loss must be 'logistic' or 'squared', got {loss!r}")
+    per = num_features // fields
+    g = torch.Generator().manual_seed(seed)
+    cols = torch.randint(0, per, (n, fields), generator=g) + torch.arange(fields) * per
+    lin = hashed_uniform(cols, 0, 2 * seed + 1).sum(1) / (fields / 3.0) ** 0.5
+    v = torch.stack([hashed_uniform(cols, f + 1, 2 * seed + 1) for f in range(k)], -1)   # [n, fields, k]
+    s = v.sum(1)
+    pairs = 0.5 * ((s * s).sum(1) - (v * v).sum((1, 2)))
+    npairs = fields * (fields - 1) / 2
+    score = lin + (2.0 / max(npairs * k / 9.0, 1e-12) ** 0.5) * pairs if fields > 1 else lin
+    if loss == "logistic":
+        labels = (torch.rand(n, generator=g) < torch.sigmoid(score)).to(torch.float32)
+    else:
+        labels = (score + 0.25 * torch.randn(n, generator=g)).to(torch.float32)
+    row_ptr = torch.arange(n + 1, dtype=torch.int64) * fields
+    return row_ptr, cols.reshape(-1).to(torch.int64), labels
