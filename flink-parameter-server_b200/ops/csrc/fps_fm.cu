@@ -17,6 +17,7 @@
 // outside [0, num_features) are skipped and raise *bad_id; the end of every example is clamped to nnz.
 #include <limits.h>
 #include "fps_common.cuh"
+#include "fps_fm_bias.cuh"
 #include "fps_launch.cuh"
 
 #define FM_THREADS 256
@@ -49,10 +50,6 @@ struct FmArgs {
   int reserve_total;         // CTA slots left free for the replica exchange
   int max_ctas;              // > 0: at most this many CTAs (tests force one-CTA grids)
 };
-
-__device__ __forceinline__ void fm_red_add1(float* p, float v) {
-  asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
-}
 
 template <typename IdT, int LPR, int VPL, int MINB, int TB, bool ONEHOT>
 __global__ void __launch_bounds__(FM_THREADS, MINB) fps_fm_kernel(const __grid_constant__ FmArgs a) {
@@ -200,44 +197,7 @@ __global__ void __launch_bounds__(FM_THREADS, MINB) fps_fm_kernel(const __grid_c
   if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
   if (bad_id && a.bad_id != nullptr) *a.bad_id = 1;
   if (a.predict_only) return;
-  // ---- per-warp sums; the last CTA steps w0 -----------------------------------------------------------------
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, o);
-    lab_acc += __shfl_xor_sync(0xffffffffu, lab_acc, o);
-    g_acc += __shfl_xor_sync(0xffffffffu, g_acc, o);
-  }
-  if ((threadIdx.x & 31) == 0 && lab_acc > 0.f) {
-    if (a.stats != nullptr) {
-      atomicAdd(a.stats + 0, loss_acc);
-      atomicAdd(a.stats + 1, lab_acc);
-    }
-    if (a.bias) {
-      atomicAdd(a.bias_acc + 0, g_acc);
-      atomicAdd(a.bias_acc + 1, (double)lab_acc);
-    }
-  }
-  if (!a.bias) return;
-  __shared__ bool s_last;
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) s_last = atomicAdd(a.bias_done, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (!s_last || threadIdx.x != 0) return;
-  __threadfence();
-  volatile double* acc = a.bias_acc;
-  const double sg = acc[0], nl = acc[1];
-  float d = 0.f;
-  if (nl > 0.0) {
-    d = -a.lr * (float)(sg / nl);
-    if (!(fabsf(d) <= 3.0e38f) && a.nan_flag != nullptr) *a.nan_flag = 1;
-    fm_red_add1(fps_row(a.tab, a.num_features), d);
-  }
-  acc[0] = 0.0;
-  acc[1] = 0.0;
-  acc[2] = (double)d;
-  acc[3] = acc[3] + (double)d;
-  *a.bias_done = 0u;
+  fps_fm_bias_tail(a, loss_acc, lab_acc, g_acc);   // per-warp sums; the last CTA steps w0
 }
 
 template <typename IdT, int LPR, int VPL, int MINB, int TB>

@@ -1,0 +1,53 @@
+// The end of a factorization-machine launch, shared by fps_fm.cu and fps_ffm.cu (DESIGN §2.15, §2.16): per-warp
+// sums of the loss, the labelled count and sum g into `stats` and `bias_acc`, then the w0 rule.  Every example reads
+// w0 as it was before the launch; the last CTA to finish (a launch counter that resets itself, behind
+// __threadfence) pushes -lr * sum g / n_labelled to column 0 of the bias row, once per launch.
+#pragma once
+#include "fps_common.cuh"
+
+__device__ __forceinline__ void fps_red_add1(float* p, float v) {
+  asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+}
+
+// Args: FmArgs or FfmArgs (stats, bias, bias_acc, bias_done, lr, nan_flag, tab, num_features).  Every thread of the
+// CTA calls it after its last example; loss_acc, lab_acc and g_acc are the thread's own sums.
+template <typename Args>
+__device__ __forceinline__ void fps_fm_bias_tail(const Args& a, float loss_acc, float lab_acc, double g_acc) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, o);
+    lab_acc += __shfl_xor_sync(0xffffffffu, lab_acc, o);
+    g_acc += __shfl_xor_sync(0xffffffffu, g_acc, o);
+  }
+  if ((threadIdx.x & 31) == 0 && lab_acc > 0.f) {
+    if (a.stats != nullptr) {
+      atomicAdd(a.stats + 0, loss_acc);
+      atomicAdd(a.stats + 1, lab_acc);
+    }
+    if (a.bias) {
+      atomicAdd(a.bias_acc + 0, g_acc);
+      atomicAdd(a.bias_acc + 1, (double)lab_acc);
+    }
+  }
+  if (!a.bias) return;
+  __shared__ bool s_last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = atomicAdd(a.bias_done, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!s_last || threadIdx.x != 0) return;
+  __threadfence();
+  volatile double* acc = a.bias_acc;
+  const double sg = acc[0], nl = acc[1];
+  float d = 0.f;
+  if (nl > 0.0) {
+    d = -a.lr * (float)(sg / nl);
+    if (!(fabsf(d) <= 3.0e38f) && a.nan_flag != nullptr) *a.nan_flag = 1;
+    fps_red_add1(fps_row(a.tab, a.num_features), d);
+  }
+  acc[0] = 0.0;
+  acc[1] = 0.0;
+  acc[2] = (double)d;
+  acc[3] = acc[3] + (double)d;
+  *a.bias_done = 0u;
+}

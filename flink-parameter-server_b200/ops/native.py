@@ -1490,6 +1490,22 @@ def fm_state(device) -> tuple:
     return torch.zeros(4, dtype=torch.float64, device=dev), torch.zeros(1, dtype=torch.int32, device=dev)
 
 
+def _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad_id, reserve_total, max_ctas):
+    """The fields :class:`FmArgsC` and :class:`FfmArgsC` share: the ``w0`` state, the counters and the grid."""
+    a.predict_only, a.bias = int(bool(predict_only)), int(bool(bias))
+    if bias and not predict_only:
+        acc, done = bias_state
+        _req(acc, "bias_acc", torch.float64); _req(done, "bias_done", torch.int32)
+        a.bias_acc, a.bias_done = acc.data_ptr(), done.data_ptr()
+    for t, name, dt in ((stats, "stats", torch.float32), (nan_flag, "nan_flag", torch.int32),
+                        (bad_id, "bad_id", torch.int32)):
+        if t is not None:
+            _req(t, name, dt)
+            setattr(a, name, t.data_ptr())
+    a.tab = tab
+    a.reserve_total, a.max_ctas = int(reserve_total), int(max_ctas)
+
+
 def fm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, vals: Optional[torch.Tensor],
             labels: Optional[torch.Tensor], pred: torch.Tensor, *, num_features: int, loss: str = "logistic",
             lr: float = 0.05, reg_linear: float = 0.0, reg_factors: float = 0.0, bias: bool = True,
@@ -1553,21 +1569,115 @@ def fm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, vals: O
     a.n, a.nnz, a.num_features = n, cols.numel(), int(num_features)
     a.dim, a.loss = int(tab.dim), FM_LOSSES[loss]
     a.lr, a.reg_linear, a.reg_factors = float(lr), float(reg_linear), float(reg_factors)
-    a.predict_only, a.bias = int(bool(predict_only)), int(bool(bias))
-    if bias and not predict_only:
-        acc, done = bias_state
-        _req(acc, "bias_acc", torch.float64); _req(done, "bias_done", torch.int32)
-        a.bias_acc, a.bias_done = acc.data_ptr(), done.data_ptr()
-    for t, name, dt in ((stats, "stats", torch.float32), (nan_flag, "nan_flag", torch.int32),
-                        (bad_id, "bad_id", torch.int32)):
-        if t is not None:
-            _req(t, name, dt)
-            setattr(a, name, t.data_ptr())
-    a.tab = tab
-    a.reserve_total, a.max_ctas = int(reserve_total), int(max_ctas)
+    _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad_id, reserve_total, max_ctas)
     if n == 0:
         return
     _check(lib().fps_fm_step(C.byref(a), _id_bytes(cols), sm_count(pred.device.index), _stream()), "fm_step")
+    _bump()
+
+
+class FfmArgsC(C.Structure):
+    """Mirror of ``struct FfmArgs`` (csrc/fps_ffm.cu)."""
+
+    _fields_ = [
+        ("row_ptr", C.c_void_p), ("cols", C.c_void_p), ("fields", C.c_void_p), ("vals", C.c_void_p),
+        ("labels", C.c_void_p), ("pred", C.c_void_p), ("stats", C.c_void_p), ("nan_flag", C.c_void_p),
+        ("bad_id", C.c_void_p), ("n", C.c_longlong), ("nnz", C.c_longlong), ("num_features", C.c_longlong),
+        ("num_fields", C.c_int), ("k", C.c_int), ("loss", C.c_int), ("lr", C.c_float), ("reg_linear", C.c_float),
+        ("reg_factors", C.c_float), ("predict_only", C.c_int), ("bias", C.c_int),
+        ("bias_acc", C.c_void_p), ("bias_done", C.c_void_p), ("tab", ShardTableC),
+        ("reserve_total", C.c_int), ("max_ctas", C.c_int),
+    ]
+
+
+FFM_MAX_FACTORS = 64
+FFM_MAX_FIELDS = 256
+
+
+def ffm_stride(num_fields: int, num_factors: int) -> int:
+    """Row length of the field-aware FM: ``[w | 0 0 0]`` and one slab of ``round_up(k, 4)`` floats per field."""
+    return 4 + int(num_fields) * 4 * -(-int(num_factors) // 4)
+
+
+def ffm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, fields: torch.Tensor,
+             vals: Optional[torch.Tensor], labels: Optional[torch.Tensor], pred: torch.Tensor, *, num_features: int,
+             num_fields: int, num_factors: int, loss: str = "logistic", lr: float = 0.05, reg_linear: float = 0.0,
+             reg_factors: float = 0.0, bias: bool = True, bias_state: Optional[tuple] = None,
+             predict_only: bool = False, stats: Optional[torch.Tensor] = None,
+             nan_flag: Optional[torch.Tensor] = None, bad_id: Optional[torch.Tensor] = None,
+             reserve_total: int = 0, max_ctas: int = 0) -> None:
+    """Fused field-aware FM step over a CSR micro-batch (csrc/fps_ffm.cu, DESIGN §2.16): one launch.
+
+    ``tab``: the model's :class:`ShardTableC`, rows ``[w | 0 0 0 | V_0 | .. | V_F-1]`` of
+    :func:`ffm_stride` floats, one slab of ``round_up(num_factors, 4)`` floats per field; id ``num_features`` is
+    the bias row (``w0`` in column 0).  ``row_ptr`` int64 ``[n + 1]``, ``cols`` int32 or int64, ``fields`` int32
+    of the same length, ``vals`` float32 or ``None`` (one-hot), ``labels`` float32 ``[n]`` (NaN: predict only;
+    ``None`` with ``predict_only``).  ``pred`` float32 ``[n]`` receives ``yhat`` from before each example's own
+    update.  ``bad_id`` is set by an entry whose feature is outside ``[0, num_features)`` or whose field is outside
+    ``[0, num_fields)`` (skipped).  ``loss``, ``stats``, ``nan_flag``, ``bias_state`` (:func:`fm_state`),
+    ``reserve_total`` and ``max_ctas`` are as in :func:`fm_step`.  Every dtype, length and argument refusal comes
+    before the library loads."""
+    if loss not in FM_LOSSES:
+        raise ValueError(f"loss must be one of {sorted(FM_LOSSES)}, got {loss!r}")
+    if not 1 <= int(num_factors) <= FFM_MAX_FACTORS:
+        raise ValueError(f"num_factors must lie in [1, {FFM_MAX_FACTORS}], got {num_factors}")
+    if not 1 <= int(num_fields) <= FFM_MAX_FIELDS:
+        raise ValueError(f"num_fields must lie in [1, {FFM_MAX_FIELDS}], got {num_fields}")
+    if int(tab.stride) != ffm_stride(num_fields, num_factors) or int(tab.dim) != int(tab.stride):
+        raise ValueError(f"the table's rows must be {ffm_stride(num_fields, num_factors)} floats "
+                         f"(4 + num_fields * round_up(num_factors, 4)), got dim {tab.dim}, stride {tab.stride}")
+    if row_ptr.dtype != torch.int64:
+        raise TypeError(f"row_ptr must be {torch.int64}, got {row_ptr.dtype}")
+    if cols.dtype not in (torch.int32, torch.int64):
+        raise TypeError(f"cols must be int32 or int64, got {cols.dtype}")
+    if fields.dtype != torch.int32:
+        raise TypeError(f"fields must be {torch.int32}, got {fields.dtype}")
+    if fields.numel() != cols.numel():
+        raise ValueError("cols and fields must have the same length")
+    if vals is not None:
+        if vals.dtype != torch.float32:
+            raise TypeError(f"vals must be {torch.float32}, got {vals.dtype}")
+        if vals.numel() != cols.numel():
+            raise ValueError("cols and vals must have the same length")
+    n = row_ptr.numel() - 1
+    if n < 0:
+        raise ValueError("row_ptr must hold n + 1 offsets")
+    if labels is None:
+        if not predict_only:
+            raise ValueError("a training step needs labels (predict_only=True predicts without)")
+    else:
+        if labels.dtype != torch.float32:
+            raise TypeError(f"labels must be {torch.float32}, got {labels.dtype}")
+        if labels.numel() != n:
+            raise ValueError(f"labels must hold one entry per example: {labels.numel()} != {n}")
+    if pred.dtype != torch.float32:
+        raise TypeError(f"pred must be {torch.float32}, got {pred.dtype}")
+    if pred.numel() != n:
+        raise ValueError(f"pred must hold one entry per example: {pred.numel()} != {n}")
+    if float(reg_linear) < 0 or float(reg_factors) < 0:
+        raise ValueError("reg_linear and reg_factors must be >= 0")
+    if int(num_features) < 0:
+        raise ValueError(f"num_features must be >= 0, got {num_features}")
+    if n >= 2 ** 31 - 1:
+        raise ValueError("a micro-batch must hold fewer than 2**31 - 1 examples")
+    if bias and not predict_only and bias_state is None:
+        raise ValueError("bias=True needs bias_state (see fm_state)")
+    _req(row_ptr, "row_ptr"); _req(cols, "cols"); _req(fields, "fields"); _req(pred, "pred")
+    if vals is not None:
+        _req(vals, "vals")
+    if labels is not None:
+        _req(labels, "labels")
+    a = FfmArgsC()
+    a.row_ptr, a.cols, a.fields, a.pred = row_ptr.data_ptr(), cols.data_ptr(), fields.data_ptr(), pred.data_ptr()
+    a.vals = vals.data_ptr() if vals is not None else None
+    a.labels = labels.data_ptr() if labels is not None else None
+    a.n, a.nnz, a.num_features = n, cols.numel(), int(num_features)
+    a.num_fields, a.k, a.loss = int(num_fields), int(num_factors), FM_LOSSES[loss]
+    a.lr, a.reg_linear, a.reg_factors = float(lr), float(reg_linear), float(reg_factors)
+    _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad_id, reserve_total, max_ctas)
+    if n == 0:
+        return
+    _check(lib().fps_ffm_step(C.byref(a), _id_bytes(cols), sm_count(pred.device.index), _stream()), "ffm_step")
     _bump()
 
 

@@ -123,3 +123,39 @@ def planted_fm(num_features: int, fields: int, k: int, n: int, seed: int = 0, lo
         labels = (score + 0.25 * torch.randn(n, generator=g)).to(torch.float32)
     row_ptr = torch.arange(n + 1, dtype=torch.int64) * fields
     return row_ptr, cols.reshape(-1).to(torch.int64), labels
+
+
+def planted_ffm(num_features: int, fields: int, k: int, n: int, seed: int = 0, loss: str = "logistic"):
+    """One-hot examples with labels from a planted field-aware factorization machine, for the FFM quality gates.
+
+    Field ``f`` owns the ids ``[f * per, (f + 1) * per)``, ``per = num_features // fields``; every example takes one
+    id per field, uniformly, in field order.  The planted model has ``w*_i = U(-1, 1)`` and one slab per (id, field)
+    ``V*[i, f]_c = U(-1, 1)`` hashed from ``(id, f, c, seed)``; its score is the linear term scaled to unit standard
+    deviation plus the pair term ``sum_{a<b} <V*[i_a, f_b], V*[i_b, f_a]>`` scaled to standard deviation 2, as in
+    :func:`planted_fm`.  ``"logistic"``: ``y ~ Bernoulli(sigmoid(score))``; ``"squared"``: ``y = score + N(0, 0.25)``.
+
+    Returns ``(row_ptr, cols, fields, labels)`` on the CPU: int64 ``[n + 1]``, int64 ``[n * fields]``, int32
+    ``[n * fields]``, float32 ``[n]``."""
+    if fields < 1 or num_features < fields or k < 1 or n < 0:
+        raise ValueError("planted_ffm needs fields >= 1, num_features >= fields, k >= 1 and n >= 0")
+    if loss not in ("logistic", "squared"):
+        raise ValueError(f"loss must be 'logistic' or 'squared', got {loss!r}")
+    per = num_features // fields
+    g = torch.Generator().manual_seed(seed)
+    cols = torch.randint(0, per, (n, fields), generator=g) + torch.arange(fields) * per
+    lin = hashed_uniform(cols, 0, 2 * seed + 1).sum(1) / (fields / 3.0) ** 0.5
+    pairs = torch.zeros(n)
+    for a in range(fields):
+        for b in range(a + 1, fields):
+            for c in range(k):
+                pairs += (hashed_uniform(cols[:, a], 1 + b * k + c, 2 * seed + 1)
+                          * hashed_uniform(cols[:, b], 1 + a * k + c, 2 * seed + 1))
+    npairs = fields * (fields - 1) / 2
+    score = lin + (2.0 / max(npairs * k / 9.0, 1e-12) ** 0.5) * pairs if fields > 1 else lin
+    if loss == "logistic":
+        labels = (torch.rand(n, generator=g) < torch.sigmoid(score)).to(torch.float32)
+    else:
+        labels = (score + 0.25 * torch.randn(n, generator=g)).to(torch.float32)
+    row_ptr = torch.arange(n + 1, dtype=torch.int64) * fields
+    field_ids = torch.arange(fields, dtype=torch.int32).repeat(n)
+    return row_ptr, cols.reshape(-1).to(torch.int64), field_ids, labels
