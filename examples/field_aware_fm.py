@@ -3,9 +3,10 @@
 Writes planted one-hot CTR-style data in libffm's text format (``label field:feature:value ...``), reads it back with
 ``read_libffm``, trains ``DeviceFieldAwareFM`` on the first part and reports the held-out AUC beside a
 ``DeviceFactorizationMachine`` with the same k and a linear model trained on the same micro-batches: the planted
-labels depend on field-aware pair interactions.
+labels depend on field-aware pair interactions.  ``--optimizer adagrad`` trains all three with libffm's AdaGrad rule
+(``--lr 0.2`` is libffm's default rate under it).
 
-    python examples/field_aware_fm.py [--k 4] [--epochs 3]
+    python examples/field_aware_fm.py [--k 4] [--epochs 3] [--optimizer sgd|adagrad] [--lr 0.1]
 """
 import argparse
 import os
@@ -23,6 +24,8 @@ def main():
     ap.add_argument("--k", type=int, default=4)
     ap.add_argument("--epochs", type=int, default=3)
     ap.add_argument("--batch", type=int, default=64)
+    ap.add_argument("--optimizer", choices=("sgd", "adagrad"), default="sgd")
+    ap.add_argument("--lr", type=float, default=0.1)
     args = ap.parse_args()
     import fps_b200  # noqa: F401
     from fps_b200.models.fm import DeviceFactorizationMachine, DeviceFieldAwareFM, read_libffm, roc_auc
@@ -44,10 +47,11 @@ def main():
     t = n_train
     for name in ("FFM", "FM", "linear"):
         if name == "FFM":
-            m = DeviceFieldAwareFM(nf, fields, args.k, learning_rate=0.1, init_range=(-0.1, 0.1), seed=5)
+            m = DeviceFieldAwareFM(nf, fields, args.k, learning_rate=args.lr, init_range=(-0.1, 0.1), seed=5,
+                                   optimizer=args.optimizer)
         else:
-            m = DeviceFactorizationMachine(nf, args.k if name == "FM" else 0, learning_rate=0.1,
-                                           init_range=(-0.1, 0.1), seed=5)
+            m = DeviceFactorizationMachine(nf, args.k if name == "FM" else 0, learning_rate=args.lr,
+                                           init_range=(-0.1, 0.1), seed=5, optimizer=args.optimizer)
         for _ in range(args.epochs):
             m.stats.zero_()
             for b0 in range(0, t, args.batch):

@@ -6,6 +6,9 @@ the global bias ``w0`` in column 0.  ``fps_fm_step`` (ops/csrc/fps_fm.cu, DESIGN
 predicts, and pushes the SGD deltas with ``red.add`` in one launch.  ``num_factors=0`` is sparse linear (squared
 loss) or logistic regression.
 
+Both train with plain SGD (``optimizer="sgd"``, the default) or libffm's element-wise AdaGrad (``"adagrad"``, DESIGN
+§2.17), whose accumulators live in a second table of the same geometry.
+
 ``DeviceFieldAwareFM`` is the field-aware FM (Juan et al. 2016, libffm): every feature keeps one latent vector per
 field, and a pair of entries interacts through the vectors each keeps for the other's field.  ``fps_ffm_step``
 (ops/csrc/fps_ffm.cu, DESIGN §2.16) runs it one warp per example, pairs spread across lanes.  ``read_libffm``
@@ -25,10 +28,16 @@ from ..store.sharded_table import ShardedTable
 from .pa.sparse import SparseVector
 
 MAX_FACTORS = native.FM_MAX_DIM - 1
+OPTIMIZERS = ("sgd", "adagrad")
+
+
+def _check_optimizer(optimizer: str) -> None:
+    if optimizer not in OPTIMIZERS:
+        raise ValueError(f"optimizer must be one of {list(OPTIMIZERS)}, got {optimizer!r}")
 
 
 def check_fm_config(num_features: int, num_factors: int, loss: str, reg_linear: float, reg_factors: float,
-                    partition: str, replica: bool) -> None:
+                    partition: str, replica: bool, optimizer: str = "sgd") -> None:
     """The refusals of :class:`DeviceFactorizationMachine`, before any device state exists."""
     if int(num_features) < 1:
         raise ValueError(f"num_features must be >= 1, got {num_features}")
@@ -44,6 +53,7 @@ def check_fm_config(num_features: int, num_factors: int, loss: str, reg_linear: 
         raise ValueError(f"partition must be 'hash' or 'range', got {partition!r}")
     if replica:
         raise ValueError("the factorization machine runs in the direct mode only: use replica=False")
+    _check_optimizer(optimizer)
 
 
 def check_fm_labels(labels: Sequence[Optional[float]], loss: str) -> np.ndarray:
@@ -74,7 +84,8 @@ def check_fm_batch(vectors: Sequence[SparseVector], labels: Sequence[Optional[fl
 
 class _FmState:
     """Observation and IO shared by the factorization machines: the device counters, the ``w0`` state, the
-    flags and the table.  Subclasses set ``table``, ``dev``, ``_stats``, ``_flags`` and ``_bias_state``."""
+    flags, the table and the AdaGrad accumulators.  Subclasses set ``table``, ``dev`` and ``optimizer`` and call
+    ``_alloc_state``."""
 
     _bad_entry = "a feature id outside [0, {nf}) was skipped"
 
@@ -82,6 +93,33 @@ class _FmState:
         self._stats = torch.zeros(2, dtype=torch.float32, device=self.dev)
         self._flags = torch.zeros(2, dtype=torch.int32, device=self.dev)   # non-finite delta, bad entry
         self._bias_state = native.fm_state(self.dev)
+        # AdaGrad's H = G - 1 per element, in the table's geometry: the zero heap is libffm's G = 1
+        self._acc = self.table.row_accumulators(self.table.stride) if self.optimizer == "adagrad" else None
+
+    @property
+    def _acc_c(self) -> Optional[native.ShardTableC]:
+        return self._acc.table_c if self._acc is not None else None
+
+    def accumulators(self) -> Tuple[List[int], np.ndarray]:
+        """AdaGrad: ``(ids, H)`` of this rank's rows, ``H`` ``[n, dim]`` in the table's row layout (the element
+        ``(id, col)`` is the accumulator of that row's column ``col``).  ``H = G - 1`` in libffm's terms."""
+        if self._acc is None:
+            raise ValueError("accumulators exist with optimizer='adagrad' only")
+        ids, H = self._acc.dump_local()
+        return ids.cpu().tolist(), H[:, :self.table.dim].cpu().numpy().astype(np.float64)
+
+    def load_accumulators(self, ids, rows) -> None:
+        """Overwrite the accumulators of ``ids`` (rows this rank owns) from ``[n, dim]`` rows, as
+        :meth:`accumulators` returns them."""
+        if self._acc is None:
+            raise ValueError("accumulators exist with optimizer='adagrad' only")
+        ids = torch.tensor(list(ids), dtype=torch.int64, device=self.dev)
+        if ids.numel() == 0:
+            return
+        rows = torch.from_numpy(np.ascontiguousarray(rows, dtype=np.float32)).reshape(ids.numel(), self.table.dim)
+        full = torch.zeros(ids.numel(), self.table.stride, dtype=torch.float32)
+        full[:, :self.table.dim] = rows
+        self._acc.load(ids, full.to(self.dev))
 
     @property
     def stats(self) -> torch.Tensor:
@@ -118,6 +156,8 @@ class _FmState:
         self.table.barrier()
 
     def close(self) -> None:
+        if self._acc is not None:
+            self._acc.close()
         self.table.close()
 
 
@@ -128,13 +168,17 @@ class DeviceFactorizationMachine(_FmState):
     example; ``loss`` ``"logistic"`` (labels 0 / 1) or ``"squared"``.  Feature rows take plain SGD with lazy L2
     (``reg_linear`` on ``w``, ``reg_factors`` on ``v``) on the rows an entry touches; ``w0`` takes one step per
     micro-batch, the mean gradient of its labelled examples, unregularised (``bias=False`` keeps it at 0).  The
-    factors start uniform in ``init_range`` as a pure function of ``(id, seed)``; ``w`` and ``w0`` start at 0."""
+    factors start uniform in ``init_range`` as a pure function of ``(id, seed)``; ``w`` and ``w0`` start at 0.
+    ``optimizer="adagrad"`` steps every element of a feature row by ``-lr * gam / sqrt(G)`` with ``G = 1 + sum gam^2``
+    over its own gradients (libffm's rule, DESIGN §2.17); ``w0`` keeps the SGD step."""
 
     def __init__(self, num_features: int, num_factors: int, *, loss: str = "logistic", learning_rate: float = 0.05,
                  reg_linear: float = 0.0, reg_factors: float = 0.0, init_range=(-0.01, 0.01), bias: bool = True,
                  partition: str = "hash", group=None, device: Optional[int] = None, seed: int = 0,
-                 replica: bool = False):
-        check_fm_config(num_features, num_factors, loss, reg_linear, reg_factors, partition, replica)
+                 replica: bool = False, optimizer: str = "sgd"):
+        check_fm_config(num_features, num_factors, loss, reg_linear, reg_factors, partition, replica,
+                        optimizer=optimizer)
+        self.optimizer = optimizer
         self.num_features, self.k = int(num_features), int(num_factors)
         self.loss, self.lr = loss, float(learning_rate)
         self.reg_linear, self.reg_factors, self.bias = float(reg_linear), float(reg_factors), bool(bias)
@@ -155,7 +199,7 @@ class DeviceFactorizationMachine(_FmState):
         native.fm_step(self.table.table_c, row_ptr, cols, vals, labels, pred, num_features=self.num_features,
                        loss=self.loss, lr=self.lr, reg_linear=self.reg_linear, reg_factors=self.reg_factors,
                        bias=self.bias, bias_state=self._bias_state, predict_only=predict_only, stats=self._stats,
-                       nan_flag=self._flags[0:1], bad_id=self._flags[1:2])
+                       nan_flag=self._flags[0:1], bad_id=self._flags[1:2], acc=self._acc_c)
         return pred
 
     def step_csr(self, row_ptr: torch.Tensor, cols: torch.Tensor, vals: Optional[torch.Tensor],
@@ -203,7 +247,7 @@ MAX_FFM_FIELDS = native.FFM_MAX_FIELDS
 
 
 def check_ffm_config(num_features: int, num_fields: int, num_factors: int, loss: str, reg_linear: float,
-                     reg_factors: float, partition: str, replica: bool) -> None:
+                     reg_factors: float, partition: str, replica: bool, optimizer: str = "sgd") -> None:
     """The refusals of :class:`DeviceFieldAwareFM`, before any device state exists."""
     if int(num_features) < 1:
         raise ValueError(f"num_features must be >= 1, got {num_features}")
@@ -222,6 +266,7 @@ def check_ffm_config(num_features: int, num_fields: int, num_factors: int, loss:
         raise ValueError(f"partition must be 'hash' or 'range', got {partition!r}")
     if replica:
         raise ValueError("the field-aware FM runs in the direct mode only: use replica=False")
+    _check_optimizer(optimizer)
 
 
 class DeviceFieldAwareFM(_FmState):
@@ -233,15 +278,19 @@ class DeviceFieldAwareFM(_FmState):
     ``w`` of every entry, ``reg_factors`` on both slabs of every pair (libffm's rule); ``w0`` takes one step per
     micro-batch, the mean gradient of its labelled examples (``bias=False`` keeps it at 0).  Row ``i`` of the table
     is ``[w_i | 0 0 0 | V_i,0 | .. | V_i,F-1]``, each slab ``round_up(k, 4)`` floats with zero padding.  The
-    factors start uniform in ``init_range`` as a pure function of ``(id, seed)``; ``w`` and ``w0`` start at 0."""
+    factors start uniform in ``init_range`` as a pure function of ``(id, seed)``; ``w`` and ``w0`` start at 0.
+    ``optimizer="adagrad"`` is libffm's training rule: every ``w`` and slab element steps by ``-lr * gam / sqrt(G)``,
+    ``G = 1 + sum gam^2`` over its own gradients (DESIGN §2.17); ``w0`` keeps the SGD step."""
 
     _bad_entry = "a feature id outside [0, {nf}) or a field outside [0, {nfields}) was skipped"
 
     def __init__(self, num_features: int, num_fields: int, num_factors: int, *, loss: str = "logistic",
                  learning_rate: float = 0.05, reg_linear: float = 0.0, reg_factors: float = 0.0,
                  init_range=(-0.01, 0.01), bias: bool = True, partition: str = "hash", group=None,
-                 device: Optional[int] = None, seed: int = 0, replica: bool = False):
-        check_ffm_config(num_features, num_fields, num_factors, loss, reg_linear, reg_factors, partition, replica)
+                 device: Optional[int] = None, seed: int = 0, replica: bool = False, optimizer: str = "sgd"):
+        check_ffm_config(num_features, num_fields, num_factors, loss, reg_linear, reg_factors, partition, replica,
+                         optimizer=optimizer)
+        self.optimizer = optimizer
         self.num_features, self.num_fields, self.k = int(num_features), int(num_fields), int(num_factors)
         self.kp = 4 * -(-self.k // 4)
         self.loss, self.lr = loss, float(learning_rate)
@@ -268,7 +317,7 @@ class DeviceFieldAwareFM(_FmState):
                         num_features=self.num_features, num_fields=self.num_fields, num_factors=self.k,
                         loss=self.loss, lr=self.lr, reg_linear=self.reg_linear, reg_factors=self.reg_factors,
                         bias=self.bias, bias_state=self._bias_state, predict_only=predict_only, stats=self._stats,
-                        nan_flag=self._flags[0:1], bad_id=self._flags[1:2])
+                        nan_flag=self._flags[0:1], bad_id=self._flags[1:2], acc=self._acc_c)
         return pred
 
     def step_csr(self, row_ptr: torch.Tensor, cols: torch.Tensor, fields: torch.Tensor,

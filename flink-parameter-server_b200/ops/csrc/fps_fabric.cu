@@ -76,11 +76,13 @@ extern "C" const char* fps_error_string(int code) {
   if (code == -1603) return "factorization machine: unknown loss code";
   if (code == -1604) return "factorization machine: n or nnz out of range";
   if (code == -1605) return "factorization machine: bias on without its accumulator";
+  if (code == -1606) return "factorization machine: AdaGrad accumulator table's geometry differs from the table's";
   if (code == -1701) return "field-aware FM: row stride is not 4 + num_fields * round_up(k, 4) floats";
   if (code == -1702) return "field-aware FM: k outside [1, 64] or num_fields outside [1, 256]";
   if (code == -1703) return "field-aware FM: unknown loss code";
   if (code == -1704) return "field-aware FM: n or nnz out of range";
   if (code == -1705) return "field-aware FM: bias on without its accumulator";
+  if (code == -1706) return "field-aware FM: AdaGrad accumulator table's geometry differs from the table's";
   if (code < 0) return "fps: invalid argument";
   return cudaGetErrorString((cudaError_t)code);
 }

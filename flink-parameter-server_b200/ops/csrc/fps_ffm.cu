@@ -17,6 +17,11 @@
 // lane-groups of Q lanes, Q = kp / 4 rounded up to a power of two, lane l holding float4 l of the pair's two slabs, TB pairs in flight per lane.
 // Pass 1 sums the pair terms and the linear term (one warp sum gives yhat); pass 2 re-pulls both slabs of each pair
 // (L2 hits) and pushes the two deltas, and pushes each entry's dw as its chunk is staged.
+//
+// AdaGrad (DESIGN §2.17): with acc.base[0] set, acc is a second table of the same geometry holding H = G - 1 per
+// element.  fps_ffm_adagrad_kernel stages each entry's H row beside its row, and in pass 2 every slab chunk and every
+// w is pulled with its H, stepped by -lr * gam / sqrtf(1 + H + gam^2) (gam: the bracket above) and pushed with
+// H += gam^2.  Pass 1 and w0 are as under SGD.
 #include <limits.h>
 #include "fps_common.cuh"
 #include "fps_fm_bias.cuh"
@@ -55,6 +60,7 @@ struct FfmArgs {
   ShardTable tab;
   int reserve_total;         // CTA slots left free for the replica exchange
   int max_ctas;              // > 0: at most this many CTAs (tests force one-CTA grids)
+  ShardTable acc;            // AdaGrad accumulators, tab's geometry; base[0] == nullptr: plain SGD
 };
 
 struct __align__(16) FfmEntry {
@@ -64,10 +70,11 @@ struct __align__(16) FfmEntry {
 };
 
 // Stage the kept entries of raw entries [j0, min(j0 + FFM_CH, e)) in CSR order into ent; returns how many.  With
-// PASS 1 each kept entry adds x w to lin; with PASS 2 it pushes dw (g and the row as re-pulled here).
-template <typename IdT, bool ONEHOT, int PASS>
+// PASS 1 each kept entry adds x w to lin; with PASS 2 it pushes dw (g and the row as re-pulled here).  With ADA the
+// entry's H row goes to hent, and PASS 2 takes the AdaGrad step on w.
+template <typename IdT, bool ONEHOT, int PASS, bool ADA = false>
 __device__ __forceinline__ int ffm_stage(const FfmArgs& a, FfmEntry* ent, long long j0, long long e, float g,
-                                         float& lin, bool& bad, bool& bad_id) {
+                                         float& lin, bool& bad, bool& bad_id, float** hent = nullptr) {
   const IdT* __restrict__ cols = reinterpret_cast<const IdT*>(a.cols);
   const int lane = threadIdx.x & 31;
   int m = 0;
@@ -77,6 +84,7 @@ __device__ __forceinline__ int ffm_stage(const FfmArgs& a, FfmEntry* ent, long l
     const long long j = j0 + h * 32 + lane;
     bool keep = false;
     float* row = nullptr;
+    float* hrow = nullptr;
     int f = 0;
     float x = 0.f;
     if (j < e) {
@@ -85,6 +93,7 @@ __device__ __forceinline__ int ffm_stage(const FfmArgs& a, FfmEntry* ent, long l
       keep = id >= 0 && id < a.num_features && f >= 0 && f < a.num_fields;
       if (keep) {
         row = fps_row_t<IdT>(a.tab, (IdT)id);
+        if constexpr (ADA) hrow = fps_row_t<IdT>(a.acc, (IdT)id);
         x = ONEHOT ? 1.f : a.vals[j];
       } else {
         bad_id = true;
@@ -97,8 +106,15 @@ __device__ __forceinline__ int ffm_stage(const FfmArgs& a, FfmEntry* ent, long l
       t.field = f;
       t.x = x;
       ent[m + __popc(mask & ((1u << lane) - 1u))] = t;
+      if constexpr (ADA) hent[m + __popc(mask & ((1u << lane) - 1u))] = hrow;
       if (PASS == 1) {
         lin += x * fps_ld_row4(row).x;
+      } else if (ADA && PASS == 2) {
+        float gg;
+        const float d = fps_adagrad1(g * x + a.reg_linear * fps_ld_row4(row).x, fps_ld_row4(hrow).x, a.lr, gg);
+        if (!(fabsf(d) + gg <= 3.0e38f)) bad = true;
+        fps_red_add1(row, d);
+        fps_red_add1(hrow, gg);
       } else if (PASS == 2) {
         const float d = -a.lr * (g * x + a.reg_linear * fps_ld_row4(row).x);
         if (!(fabsf(d) <= 3.0e38f)) bad = true;
@@ -270,10 +286,178 @@ __global__ void __launch_bounds__(FFM_THREADS, MINB) fps_ffm_kernel(const __grid
   fps_fm_bias_tail(a, loss_acc, lab_acc, g_acc);
 }
 
-template <typename IdT, int Q, int MINB, int TB>
+template <typename IdT, int Q, int MINB, int TB, bool ONEHOT>
+__global__ void __launch_bounds__(FFM_THREADS, MINB) fps_ffm_adagrad_kernel(const __grid_constant__ FfmArgs a) {
+  constexpr int P = 32 / Q;        // pairs per warp per step
+  __shared__ FfmEntry s_ent[FFM_WARPS][2][FFM_CH];
+  __shared__ float* s_hrow[FFM_WARPS][2][FFM_CH];   // each staged entry's H row
+  const int lane = threadIdx.x & 31;
+  const int li = lane & (Q - 1);   // my float4 of the slab
+  const int gi = lane / Q;         // my lane-group
+  FfmEntry* entA = s_ent[threadIdx.x >> 5][0];
+  FfmEntry* entB = s_ent[threadIdx.x >> 5][1];
+  float** hA = s_hrow[threadIdx.x >> 5][0];
+  float** hB = s_hrow[threadIdx.x >> 5][1];
+  const int kp = 4 * ((a.k + 3) / 4);
+  // columns of my float4 inside the slab that hold factors: [k, kp) is padding and receives exact zeros; a lane
+  // whose float4 lies past the slab (kp / 4 < Q) neither pulls nor pushes
+  const int c0 = 4 * li;
+  const bool on = c0 < kp;
+  const bool m0 = c0 < a.k, m1 = c0 + 1 < a.k, m2 = c0 + 2 < a.k, m3 = c0 + 3 < a.k;
+  const float w0 = a.bias ? fps_ld_row4(fps_row(a.tab, a.num_features)).x : 0.f;
+
+  const long long warp = (blockIdx.x * (long long)FFM_THREADS + threadIdx.x) >> 5;
+  const long long n_warps = ((long long)gridDim.x * FFM_THREADS) >> 5;
+  float loss_acc = 0.f, lab_acc = 0.f;
+  double g_acc = 0.0;
+  bool bad = false, bad_id = false;
+
+  // one example per warp: the trip count is warp-uniform
+  for (long long ex = warp; ex < a.n; ex += n_warps) {
+    long long e = a.row_ptr[ex + 1];
+    long long b = a.row_ptr[ex];
+    if (e > a.nnz) e = a.nnz;
+    if (b < 0) b = 0;
+    if (b > e) b = e;
+    const int nc = (int)((e - b + FFM_CH - 1) / FFM_CH);
+    // ---- pass 1: linear term and pair terms --------------------------------------------------------------
+    float acc = 0.f, lin = 0.f;
+    for (int A = 0; A < nc; ++A) {
+      const int mA = ffm_stage<IdT, ONEHOT, 1>(a, entA, b + (long long)A * FFM_CH, e, 0.f, lin, bad, bad_id);
+      for (int B = A; B < nc; ++B) {
+        float unused = 0.f;
+        const int mB = B == A ? mA : ffm_stage<IdT, ONEHOT, 0>(a, entB, b + (long long)B * FFM_CH, e, 0.f, unused,
+                                                               bad, bad_id);
+        const FfmEntry* eb = B == A ? entA : entB;
+        const int np = B == A ? mA * (mA - 1) / 2 : mA * mB;
+        for (int p0 = 0; p0 < np; p0 += P * TB) {
+          float4 ra[TB], rb[TB];
+          float xx[TB];
+#pragma unroll
+          for (int t = 0; t < TB; ++t) {
+            const int p = p0 + t * P + gi;
+            xx[t] = 0.f;
+            ra[t] = make_float4(0.f, 0.f, 0.f, 0.f);
+            rb[t] = ra[t];
+            if (p < np && on) {
+              int ia, ib;
+              ffm_pair(p, B == A, mB, ia, ib);
+              const FfmEntry ea = entA[ia], ebb = eb[ib];
+              xx[t] = ea.x * ebb.x;
+              ra[t] = fps_ld_row4(ea.row + 4 + ebb.field * kp + c0);   // V[i_a, f_b]
+              rb[t] = fps_ld_row4(ebb.row + 4 + ea.field * kp + c0);   // V[i_b, f_a]
+            }
+          }
+#pragma unroll
+          for (int t = 0; t < TB; ++t)
+            acc += xx[t] * (ra[t].x * rb[t].x + ra[t].y * rb[t].y + ra[t].z * rb[t].z + ra[t].w * rb[t].w);
+        }
+      }
+    }
+    const float yhat = w0 + fps_group_sum<32>(lin + acc);
+    if (lane == 0) a.pred[ex] = yhat;
+    if (a.predict_only) continue;
+    const float y = a.labels[ex];
+    if (y != y) continue;
+    float g;
+    if (a.loss == FFM_LOGISTIC) {
+      g = 1.f / (1.f + expf(-yhat)) - y;
+      if (lane == 0) loss_acc += fmaxf(yhat, 0.f) + log1pf(expf(-fabsf(yhat))) - y * yhat;
+    } else {
+      g = yhat - y;
+      if (lane == 0) loss_acc += g * g;
+    }
+    if (lane == 0) {
+      lab_acc += 1.f;
+      g_acc += (double)g;
+    }
+    // ---- pass 2: re-pull both slabs of every pair with their H, push the deltas and gam^2; w as staged ------
+    for (int A = 0; A < nc; ++A) {
+      float unused = 0.f;
+      const int mA = ffm_stage<IdT, ONEHOT, 2, true>(a, entA, b + (long long)A * FFM_CH, e, g, unused, bad, bad_id,
+                                                      hA);
+      for (int B = A; B < nc; ++B) {
+        const int mB = B == A ? mA : ffm_stage<IdT, ONEHOT, 0, true>(a, entB, b + (long long)B * FFM_CH, e, 0.f,
+                                                                     unused, bad, bad_id, hB);
+        const FfmEntry* eb = B == A ? entA : entB;
+        float* const* hb_ = B == A ? hA : hB;
+        const int np = B == A ? mA * (mA - 1) / 2 : mA * mB;
+        for (int p0 = 0; p0 < np; p0 += P * TB) {
+          float4 ra[TB], rb[TB], ha[TB], hb[TB];
+          float* pa[TB];
+          float* pb[TB];
+          float* qa[TB];
+          float* qb[TB];
+          float cc[TB];
+#pragma unroll
+          for (int t = 0; t < TB; ++t) {
+            const int p = p0 + t * P + gi;
+            pa[t] = nullptr;
+            pb[t] = nullptr;
+            qa[t] = nullptr;
+            qb[t] = nullptr;
+            cc[t] = 0.f;
+            ra[t] = make_float4(0.f, 0.f, 0.f, 0.f);
+            rb[t] = ra[t];
+            ha[t] = ra[t];
+            hb[t] = ra[t];
+            if (p < np && on) {
+              int ia, ib;
+              ffm_pair(p, B == A, mB, ia, ib);
+              const FfmEntry ea = entA[ia], ebb = eb[ib];
+              cc[t] = g * (ea.x * ebb.x);
+              const int oa = 4 + ebb.field * kp + c0, ob = 4 + ea.field * kp + c0;
+              pa[t] = ea.row + oa;
+              pb[t] = ebb.row + ob;
+              qa[t] = hA[ia] + oa;
+              qb[t] = hb_[ib] + ob;
+              ra[t] = fps_ld_row4(pa[t]);
+              rb[t] = fps_ld_row4(pb[t]);
+              ha[t] = fps_ld_row4(qa[t]);
+              hb[t] = fps_ld_row4(qb[t]);
+            }
+          }
+#pragma unroll
+          for (int t = 0; t < TB; ++t) {
+            if (pa[t] == nullptr) continue;
+            const float c = cc[t], rv = a.reg_factors;
+            float4 ga, gb, gga, ggb;
+            ga.x = m0 ? c * rb[t].x + rv * ra[t].x : 0.f;
+            ga.y = m1 ? c * rb[t].y + rv * ra[t].y : 0.f;
+            ga.z = m2 ? c * rb[t].z + rv * ra[t].z : 0.f;
+            ga.w = m3 ? c * rb[t].w + rv * ra[t].w : 0.f;
+            gb.x = m0 ? c * ra[t].x + rv * rb[t].x : 0.f;
+            gb.y = m1 ? c * ra[t].y + rv * rb[t].y : 0.f;
+            gb.z = m2 ? c * ra[t].z + rv * rb[t].z : 0.f;
+            gb.w = m3 ? c * ra[t].w + rv * rb[t].w : 0.f;
+            const float4 da = fps_adagrad4(ga, ha[t], a.lr, gga);
+            const float4 db = fps_adagrad4(gb, hb[t], a.lr, ggb);
+            if (!(fabsf(da.x) + fabsf(da.y) + fabsf(da.z) + fabsf(da.w) + fabsf(db.x) + fabsf(db.y) + fabsf(db.z) +
+                      fabsf(db.w) + gga.x + gga.y + gga.z + gga.w + ggb.x + ggb.y + ggb.z + ggb.w <= 3.0e38f))
+              bad = true;
+            fps_red_add4(pa[t], da);
+            fps_red_add4(pb[t], db);
+            fps_red_add4(qa[t], gga);
+            fps_red_add4(qb[t], ggb);
+          }
+        }
+      }
+    }
+  }
+  if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
+  if (bad_id && a.bad_id != nullptr) *a.bad_id = 1;
+  if (a.predict_only) return;
+  fps_fm_bias_tail(a, loss_acc, lab_acc, g_acc);
+}
+
+template <typename IdT, int Q, int MINB, int TB, bool ADA>
 static int launch_ffm(const FfmArgs& a, int num_sms, cudaStream_t stream) {
-  void (*kern)(const FfmArgs) = a.vals == nullptr ? fps_ffm_kernel<IdT, Q, MINB, TB, true>
-                                                  : fps_ffm_kernel<IdT, Q, MINB, TB, false>;
+  void (*kern)(const FfmArgs);
+  if constexpr (ADA)
+    kern = a.vals == nullptr ? fps_ffm_adagrad_kernel<IdT, Q, MINB, TB, true>
+                             : fps_ffm_adagrad_kernel<IdT, Q, MINB, TB, false>;
+  else
+    kern = a.vals == nullptr ? fps_ffm_kernel<IdT, Q, MINB, TB, true> : fps_ffm_kernel<IdT, Q, MINB, TB, false>;
   long long blocks = fps_row_grid(kern, FFM_THREADS, FFM_WARPS, num_sms, a.reserve_total, 0, 1, a.n, 1);
   if (a.max_ctas > 0 && blocks > a.max_ctas) blocks = a.max_ctas;
   kern<<<(int)blocks, FFM_THREADS, 0, stream>>>(a);
@@ -281,14 +465,17 @@ static int launch_ffm(const FfmArgs& a, int num_sms, cudaStream_t stream) {
 }
 
 // Q = kp / 4 rounded up to a power of two lanes per pair; MINB keeps every instantiation free of spills (ptxas -v, DESIGN §3).
-template <typename IdT>
+// AdaGrad holds two more float4 and two more pointers per pair in flight, so it runs TB = ADA_TB pairs per lane.
+#define FFM_ADA_TB 2
+template <typename IdT, bool ADA>
 static int ffm_dispatch(const FfmArgs& a, int num_sms, cudaStream_t s) {
+  constexpr int TB = ADA ? FFM_ADA_TB : 4;
   const int q = (a.k + 3) / 4;
-  if (q <= 1) return launch_ffm<IdT, 1, 2, 4>(a, num_sms, s);
-  if (q <= 2) return launch_ffm<IdT, 2, 2, 4>(a, num_sms, s);
-  if (q <= 4) return launch_ffm<IdT, 4, 2, 4>(a, num_sms, s);
-  if (q <= 8) return launch_ffm<IdT, 8, 2, 4>(a, num_sms, s);
-  return launch_ffm<IdT, 16, 2, 4>(a, num_sms, s);
+  if (q <= 1) return launch_ffm<IdT, 1, 2, TB, ADA>(a, num_sms, s);
+  if (q <= 2) return launch_ffm<IdT, 2, 2, TB, ADA>(a, num_sms, s);
+  if (q <= 4) return launch_ffm<IdT, 4, 2, TB, ADA>(a, num_sms, s);
+  if (q <= 8) return launch_ffm<IdT, 8, 2, TB, ADA>(a, num_sms, s);
+  return launch_ffm<IdT, 16, 2, TB, ADA>(a, num_sms, s);
 }
 
 extern "C" int fps_ffm_step(const FfmArgs* args, int id_bytes, int num_sms, cudaStream_t stream) {
@@ -298,8 +485,13 @@ extern "C" int fps_ffm_step(const FfmArgs* args, int id_bytes, int num_sms, cuda
   if (a.loss != FFM_LOGISTIC && a.loss != FFM_SQUARED) return -1703;
   if (a.n < 0 || a.n >= INT_MAX || a.nnz < 0 || a.num_features < 0) return -1704;
   if (a.bias && !a.predict_only && (a.bias_acc == nullptr || a.bias_done == nullptr)) return -1705;
+  const bool ada = a.acc.base[0] != nullptr;
+  if (ada && !fps_same_geometry(a.acc, a.tab)) return -1706;
   if (a.n == 0) return 0;
-  if (id_bytes == 4) return ffm_dispatch<int>(a, num_sms, stream);
-  if (id_bytes == 8) return ffm_dispatch<long long>(a, num_sms, stream);
+  // predictions come from the AdaGrad kernel too (its pass 1 sums in the same blocks as its training step); with
+  // predict_only it never reaches H
+  if (id_bytes == 4) return ada ? ffm_dispatch<int, true>(a, num_sms, stream) : ffm_dispatch<int, false>(a, num_sms, stream);
+  if (id_bytes == 8)
+    return ada ? ffm_dispatch<long long, true>(a, num_sms, stream) : ffm_dispatch<long long, false>(a, num_sms, stream);
   return -1001;
 }

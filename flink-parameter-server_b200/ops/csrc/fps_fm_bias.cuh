@@ -9,6 +9,24 @@ __device__ __forceinline__ void fps_red_add1(float* p, float v) {
   asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
 }
 
+// An AdaGrad accumulator table (DESIGN §2.17) must address H exactly as the parameter table addresses the row.
+__host__ __device__ inline bool fps_same_geometry(const ShardTable& acc, const ShardTable& tab) {
+  return acc.stride == tab.stride && acc.dim == tab.dim && acc.rows_per_shard == tab.rows_per_shard &&
+         acc.div == tab.div && acc.num_shards == tab.num_shards && acc.mode == tab.mode;
+}
+
+// libffm's AdaGrad step of one element (DESIGN §2.17): gam is what plain SGD would scale by -lr, h the element's
+// H = G - 1 as pulled.  Returns the delta; gg receives gam^2, the push to H.  sqrtf and the division are IEEE
+// round-to-nearest (no fast-math), so the replay's error model charges one rounding each.
+__device__ __forceinline__ float fps_adagrad1(float gam, float h, float lr, float& gg) {
+  gg = gam * gam;
+  return -lr * gam / sqrtf(1.f + h + gg);
+}
+__device__ __forceinline__ float4 fps_adagrad4(float4 gam, float4 h, float lr, float4& gg) {
+  return make_float4(fps_adagrad1(gam.x, h.x, lr, gg.x), fps_adagrad1(gam.y, h.y, lr, gg.y),
+                     fps_adagrad1(gam.z, h.z, lr, gg.z), fps_adagrad1(gam.w, h.w, lr, gg.w));
+}
+
 // Args: FmArgs or FfmArgs (stats, bias, bias_acc, bias_done, lr, nan_flag, tab, num_features).  Every thread of the
 // CTA calls it after its last example; loss_acc, lab_acc and g_acc are the thread's own sums.
 template <typename Args>

@@ -1474,7 +1474,7 @@ class FmArgsC(C.Structure):
         ("dim", C.c_int), ("loss", C.c_int), ("lr", C.c_float), ("reg_linear", C.c_float),
         ("reg_factors", C.c_float), ("predict_only", C.c_int), ("bias", C.c_int), ("pad_", C.c_int),
         ("bias_acc", C.c_void_p), ("bias_done", C.c_void_p), ("tab", ShardTableC),
-        ("reserve_total", C.c_int), ("max_ctas", C.c_int),
+        ("reserve_total", C.c_int), ("max_ctas", C.c_int), ("acc", ShardTableC),
     ]
 
 
@@ -1490,13 +1490,31 @@ def fm_state(device) -> tuple:
     return torch.zeros(4, dtype=torch.float64, device=dev), torch.zeros(1, dtype=torch.int32, device=dev)
 
 
-def _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad_id, reserve_total, max_ctas):
-    """The fields :class:`FmArgsC` and :class:`FfmArgsC` share: the ``w0`` state, the counters and the grid."""
+def _check_fm_acc(acc, tab) -> None:
+    """An AdaGrad accumulator table must have the parameter table's geometry: ``H`` of element ``(id, col)`` sits at
+    the row's slot and column (DESIGN §2.17)."""
+    if acc is None:
+        return
+    if not isinstance(acc, ShardTableC):
+        raise TypeError(f"acc must be a ShardTableC or None, got {type(acc).__name__}")
+    if not acc.base[0]:
+        raise ValueError("acc has no shard 0 (a null base pointer would select plain SGD)")
+    geo = ("stride", "dim", "rows_per_shard", "div", "num_shards", "mode")
+    mine, theirs = tuple(int(getattr(acc, f)) for f in geo), tuple(int(getattr(tab, f)) for f in geo)
+    if mine != theirs:
+        raise ValueError(f"the accumulator table's geometry (stride, dim, rows_per_shard, div, shards, mode) {mine} "
+                         f"differs from the parameter table's {theirs}")
+
+
+def _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad_id, reserve_total, max_ctas,
+                    acc=None):
+    """The fields :class:`FmArgsC` and :class:`FfmArgsC` share: the ``w0`` state, the counters, the grid and the
+    AdaGrad accumulators."""
     a.predict_only, a.bias = int(bool(predict_only)), int(bool(bias))
     if bias and not predict_only:
-        acc, done = bias_state
-        _req(acc, "bias_acc", torch.float64); _req(done, "bias_done", torch.int32)
-        a.bias_acc, a.bias_done = acc.data_ptr(), done.data_ptr()
+        bias_acc, done = bias_state
+        _req(bias_acc, "bias_acc", torch.float64); _req(done, "bias_done", torch.int32)
+        a.bias_acc, a.bias_done = bias_acc.data_ptr(), done.data_ptr()
     for t, name, dt in ((stats, "stats", torch.float32), (nan_flag, "nan_flag", torch.int32),
                         (bad_id, "bad_id", torch.int32)):
         if t is not None:
@@ -1504,6 +1522,8 @@ def _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad
             setattr(a, name, t.data_ptr())
     a.tab = tab
     a.reserve_total, a.max_ctas = int(reserve_total), int(max_ctas)
+    if acc is not None:
+        a.acc = acc
 
 
 def fm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, vals: Optional[torch.Tensor],
@@ -1511,7 +1531,7 @@ def fm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, vals: O
             lr: float = 0.05, reg_linear: float = 0.0, reg_factors: float = 0.0, bias: bool = True,
             bias_state: Optional[tuple] = None, predict_only: bool = False, stats: Optional[torch.Tensor] = None,
             nan_flag: Optional[torch.Tensor] = None, bad_id: Optional[torch.Tensor] = None,
-            reserve_total: int = 0, max_ctas: int = 0) -> None:
+            reserve_total: int = 0, max_ctas: int = 0, acc: Optional[ShardTableC] = None) -> None:
     """Fused factorization-machine step over a CSR micro-batch (csrc/fps_fm.cu, DESIGN §2.15): one launch.
 
     ``tab``: the model's :class:`ShardTableC`, rows ``[w | v_1 .. v_k | 0]`` of ``dim = 1 + k`` floats, id
@@ -1522,9 +1542,13 @@ def fm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, vals: O
     ``[2]``) accumulates the loss and the labelled examples; ``nan_flag`` is set by a non-finite delta, ``bad_id``
     by an entry outside ``[0, num_features)`` (skipped).  With ``bias``, ``bias_state`` (:func:`fm_state`) carries
     the per-launch ``w0`` step: ``w0 -= lr * sum g / n_labelled``, pushed by the last CTA.  ``max_ctas`` > 0 caps
-    the grid.  Every dtype, length and argument refusal comes before the library loads."""
+    the grid.  ``acc``: a :class:`ShardTableC` of ``tab``'s geometry holding AdaGrad's ``H`` per element (DESIGN
+    §2.17); the feature rows then step by ``-lr * gam / sqrt(1 + H + gam^2)`` and ``H += gam^2``, where ``gam`` is
+    the SGD gradient with its L2 term (``w0`` keeps the SGD rule; ``predict_only`` leaves ``H`` alone).  ``None``:
+    plain SGD.  Every dtype, length and argument refusal comes before the library loads."""
     if loss not in FM_LOSSES:
         raise ValueError(f"loss must be one of {sorted(FM_LOSSES)}, got {loss!r}")
+    _check_fm_acc(acc, tab)
     if row_ptr.dtype != torch.int64:
         raise TypeError(f"row_ptr must be {torch.int64}, got {row_ptr.dtype}")
     if cols.dtype not in (torch.int32, torch.int64):
@@ -1569,7 +1593,7 @@ def fm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, vals: O
     a.n, a.nnz, a.num_features = n, cols.numel(), int(num_features)
     a.dim, a.loss = int(tab.dim), FM_LOSSES[loss]
     a.lr, a.reg_linear, a.reg_factors = float(lr), float(reg_linear), float(reg_factors)
-    _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad_id, reserve_total, max_ctas)
+    _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad_id, reserve_total, max_ctas, acc)
     if n == 0:
         return
     _check(lib().fps_fm_step(C.byref(a), _id_bytes(cols), sm_count(pred.device.index), _stream()), "fm_step")
@@ -1586,7 +1610,7 @@ class FfmArgsC(C.Structure):
         ("num_fields", C.c_int), ("k", C.c_int), ("loss", C.c_int), ("lr", C.c_float), ("reg_linear", C.c_float),
         ("reg_factors", C.c_float), ("predict_only", C.c_int), ("bias", C.c_int),
         ("bias_acc", C.c_void_p), ("bias_done", C.c_void_p), ("tab", ShardTableC),
-        ("reserve_total", C.c_int), ("max_ctas", C.c_int),
+        ("reserve_total", C.c_int), ("max_ctas", C.c_int), ("acc", ShardTableC),
     ]
 
 
@@ -1605,7 +1629,7 @@ def ffm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, fields
              reg_factors: float = 0.0, bias: bool = True, bias_state: Optional[tuple] = None,
              predict_only: bool = False, stats: Optional[torch.Tensor] = None,
              nan_flag: Optional[torch.Tensor] = None, bad_id: Optional[torch.Tensor] = None,
-             reserve_total: int = 0, max_ctas: int = 0) -> None:
+             reserve_total: int = 0, max_ctas: int = 0, acc: Optional[ShardTableC] = None) -> None:
     """Fused field-aware FM step over a CSR micro-batch (csrc/fps_ffm.cu, DESIGN §2.16): one launch.
 
     ``tab``: the model's :class:`ShardTableC`, rows ``[w | 0 0 0 | V_0 | .. | V_F-1]`` of
@@ -1615,8 +1639,8 @@ def ffm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, fields
     ``None`` with ``predict_only``).  ``pred`` float32 ``[n]`` receives ``yhat`` from before each example's own
     update.  ``bad_id`` is set by an entry whose feature is outside ``[0, num_features)`` or whose field is outside
     ``[0, num_fields)`` (skipped).  ``loss``, ``stats``, ``nan_flag``, ``bias_state`` (:func:`fm_state`),
-    ``reserve_total`` and ``max_ctas`` are as in :func:`fm_step`.  Every dtype, length and argument refusal comes
-    before the library loads."""
+    ``reserve_total``, ``max_ctas`` and ``acc`` (AdaGrad on ``w`` and on both slabs of every pair, DESIGN §2.17) are
+    as in :func:`fm_step`.  Every dtype, length and argument refusal comes before the library loads."""
     if loss not in FM_LOSSES:
         raise ValueError(f"loss must be one of {sorted(FM_LOSSES)}, got {loss!r}")
     if not 1 <= int(num_factors) <= FFM_MAX_FACTORS:
@@ -1626,6 +1650,7 @@ def ffm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, fields
     if int(tab.stride) != ffm_stride(num_fields, num_factors) or int(tab.dim) != int(tab.stride):
         raise ValueError(f"the table's rows must be {ffm_stride(num_fields, num_factors)} floats "
                          f"(4 + num_fields * round_up(num_factors, 4)), got dim {tab.dim}, stride {tab.stride}")
+    _check_fm_acc(acc, tab)
     if row_ptr.dtype != torch.int64:
         raise TypeError(f"row_ptr must be {torch.int64}, got {row_ptr.dtype}")
     if cols.dtype not in (torch.int32, torch.int64):
@@ -1674,7 +1699,7 @@ def ffm_step(tab: ShardTableC, row_ptr: torch.Tensor, cols: torch.Tensor, fields
     a.n, a.nnz, a.num_features = n, cols.numel(), int(num_features)
     a.num_fields, a.k, a.loss = int(num_fields), int(num_factors), FM_LOSSES[loss]
     a.lr, a.reg_linear, a.reg_factors = float(lr), float(reg_linear), float(reg_factors)
-    _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad_id, reserve_total, max_ctas)
+    _fm_common_args(a, tab, bias, bias_state, predict_only, stats, nan_flag, bad_id, reserve_total, max_ctas, acc)
     if n == 0:
         return
     _check(lib().fps_ffm_step(C.byref(a), _id_bytes(cols), sm_count(pred.device.index), _stream()), "ffm_step")

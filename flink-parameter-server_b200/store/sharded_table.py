@@ -216,32 +216,41 @@ class ShardedTable:
     def close(self) -> None:
         self.heap.close()
 
-    def row_accumulators(self) -> "RowAccumulators":
-        """One zeroed fp32 per row of this table, partitioned exactly like it (row-wise AdaGrad state)."""
-        return RowAccumulators(self)
+    def row_accumulators(self, width: int = 1) -> "RowAccumulators":
+        """Zeroed fp32 optimizer state partitioned exactly like this table: one per row (``width=1``, row-wise
+        AdaGrad) or one per element (``width=stride``, element-wise AdaGrad)."""
+        return RowAccumulators(self, width)
 
 
 class RowAccumulators:
-    """Per-row optimizer state of a :class:`ShardedTable`: a ``[rows_per_shard]`` fp32 block per shard in its
-    own symmetric heap, so peers read and reduce it the way they reach the rows.  ``table_c`` addresses it
-    with the table's partitioning and stride 1; ``local`` is this rank's block."""
+    """Optimizer state of a :class:`ShardedTable`: a ``[rows_per_shard]`` (``width=1``: one per row) or
+    ``[rows_per_shard, stride]`` (``width=stride``: one per element, at its parameter's slot and column) fp32 block
+    per shard in its own symmetric heap, so peers read and reduce it the way they reach the rows.  ``table_c``
+    addresses it with the table's partitioning (stride 1, or the table's dim and stride); ``local`` is this rank's
+    block."""
 
-    def __init__(self, table: ShardedTable):
+    def __init__(self, table: ShardedTable, width: int = 1):
+        if int(width) not in (1, table.stride):
+            raise ValueError(f"width must be 1 (per row) or the table's stride {table.stride} (per element), "
+                             f"got {width}")
         self.table = table
-        self.heap = SymmetricHeap(table.rows_per_shard * 4, group=table.group, device=table.device,
+        self.width = int(width)
+        self.heap = SymmetricHeap(table.rows_per_shard * self.width * 4, group=table.group, device=table.device,
                                   mode=table.heap.mode)
-        self.local = self.heap.local_tensor((table.rows_per_shard,), torch.float32)
+        shape = (table.rows_per_shard,) if self.width == 1 else (table.rows_per_shard, self.width)
+        self.local = self.heap.local_tensor(shape, torch.float32)
         src = table.table_c
         tc = native.ShardTableC()
         for r in range(table.n_shards):
             tc.base[r] = self.heap.peer_ptrs[r]
         tc.rows_per_shard, tc.div, tc.num_shards = src.rows_per_shard, src.div, src.num_shards
-        tc.dim, tc.stride, tc.mode, tc.shard_shift, tc.lut = 1, 1, src.mode, src.shard_shift, src.lut
+        tc.dim, tc.stride = (1, 1) if self.width == 1 else (src.dim, src.stride)
+        tc.mode, tc.shard_shift, tc.lut = src.mode, src.shard_shift, src.lut
         self.table_c = tc
         self.heap.barrier()
 
     def dump_local(self) -> Tuple[torch.Tensor, torch.Tensor]:
-        """(ids, accumulators) of the local shard's valid rows."""
+        """(ids, accumulators) of the local shard's valid rows (``[n]``, or ``[n, stride]`` per element)."""
         torch.cuda.synchronize(self.table.device)
         ids = self.table.local_ids()
         sel = (ids < self.table.num_ids).nonzero(as_tuple=True)[0]
