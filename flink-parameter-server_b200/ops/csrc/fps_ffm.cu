@@ -19,9 +19,10 @@
 // (L2 hits) and pushes the two deltas, and pushes each entry's dw as its chunk is staged.
 //
 // AdaGrad (DESIGN §2.17): with acc.base[0] set, acc is a second table of the same geometry holding H = G - 1 per
-// element.  fps_ffm_adagrad_kernel stages each entry's H row beside its row, and in pass 2 every slab chunk and every
-// w is pulled with its H, stepped by -lr * gam / sqrtf(1 + H + gam^2) (gam: the bracket above) and pushed with
-// H += gam^2.  Pass 1 and w0 are as under SGD.
+// element, and the step launches fps_ffm_kernel with ADA set.  Pass 1 and w0 are shared with SGD; pass 2 stages each
+// entry's H row beside its row, and every slab chunk and every w is pulled with its H, stepped by
+// -lr * gam / sqrtf(1 + H + gam^2) (gam: the bracket above) and pushed with H += gam^2.  The two pass 2 tile loops
+// stay apart, as in fps_fm.cu.
 #include <limits.h>
 #include "fps_common.cuh"
 #include "fps_fm_bias.cuh"
@@ -32,7 +33,6 @@
 #define FFM_CH 64          // entries per staged chunk
 #define FFM_MAX_K 64
 #define FFM_MAX_FIELDS 256
-enum FfmLoss : int { FFM_LOGISTIC = 0, FFM_SQUARED = 1 };
 
 struct FfmArgs {
   const long long* row_ptr;  // [n + 1]
@@ -49,7 +49,7 @@ struct FfmArgs {
   long long num_features;    // the bias row's id
   int num_fields;            // F
   int k;                     // factors per slab; slabs are round_up(k, 4) floats apart
-  int loss;                  // FfmLoss
+  int loss;                  // FmLoss
   float lr;
   float reg_linear;
   float reg_factors;
@@ -142,10 +142,11 @@ __device__ __forceinline__ void ffm_pair(int p, bool same, int mB, int& ia, int&
   }
 }
 
-template <typename IdT, int Q, int MINB, int TB, bool ONEHOT>
+template <typename IdT, int Q, int MINB, int TB, bool ONEHOT, bool ADA>
 __global__ void __launch_bounds__(FFM_THREADS, MINB) fps_ffm_kernel(const __grid_constant__ FfmArgs a) {
   constexpr int P = 32 / Q;        // pairs per warp per step
   __shared__ FfmEntry s_ent[FFM_WARPS][2][FFM_CH];
+  __shared__ float* s_hrow[ADA ? FFM_WARPS : 1][2][FFM_CH];   // each staged entry's H row (AdaGrad)
   const int lane = threadIdx.x & 31;
   const int li = lane & (Q - 1);   // my float4 of the slab
   const int gi = lane / Q;         // my lane-group
@@ -213,7 +214,7 @@ __global__ void __launch_bounds__(FFM_THREADS, MINB) fps_ffm_kernel(const __grid
     const float y = a.labels[ex];
     if (y != y) continue;
     float g;
-    if (a.loss == FFM_LOGISTIC) {
+    if (a.loss == FM_LOGISTIC) {
       g = 1.f / (1.f + expf(-yhat)) - y;
       if (lane == 0) loss_acc += fmaxf(yhat, 0.f) + log1pf(expf(-fabsf(yhat))) - y * yhat;
     } else {
@@ -224,240 +225,145 @@ __global__ void __launch_bounds__(FFM_THREADS, MINB) fps_ffm_kernel(const __grid
       lab_acc += 1.f;
       g_acc += (double)g;
     }
-    // ---- pass 2: re-pull both slabs of every pair, push the deltas; dw as each A chunk is staged -----------
-    for (int A = 0; A < nc; ++A) {
-      float unused = 0.f;
-      const int mA = ffm_stage<IdT, ONEHOT, 2>(a, entA, b + (long long)A * FFM_CH, e, g, unused, bad, bad_id);
-      for (int B = A; B < nc; ++B) {
-        const int mB = B == A ? mA : ffm_stage<IdT, ONEHOT, 0>(a, entB, b + (long long)B * FFM_CH, e, 0.f, unused,
-                                                               bad, bad_id);
-        const FfmEntry* eb = B == A ? entA : entB;
-        const int np = B == A ? mA * (mA - 1) / 2 : mA * mB;
-        for (int p0 = 0; p0 < np; p0 += P * TB) {
-          float4 ra[TB], rb[TB];
-          float* pa[TB];
-          float* pb[TB];
-          float cc[TB];
-#pragma unroll
-          for (int t = 0; t < TB; ++t) {
-            const int p = p0 + t * P + gi;
-            pa[t] = nullptr;
-            pb[t] = nullptr;
-            cc[t] = 0.f;
-            ra[t] = make_float4(0.f, 0.f, 0.f, 0.f);
-            rb[t] = ra[t];
-            if (p < np && on) {
-              int ia, ib;
-              ffm_pair(p, B == A, mB, ia, ib);
-              const FfmEntry ea = entA[ia], ebb = eb[ib];
-              cc[t] = g * (ea.x * ebb.x);
-              pa[t] = ea.row + 4 + ebb.field * kp + c0;
-              pb[t] = ebb.row + 4 + ea.field * kp + c0;
-              ra[t] = fps_ld_row4(pa[t]);
-              rb[t] = fps_ld_row4(pb[t]);
-            }
-          }
-#pragma unroll
-          for (int t = 0; t < TB; ++t) {
-            if (pa[t] == nullptr) continue;
-            const float c = cc[t], rv = a.reg_factors, lr = a.lr;
-            float4 da, db;
-            da.x = m0 ? -lr * (c * rb[t].x + rv * ra[t].x) : 0.f;
-            da.y = m1 ? -lr * (c * rb[t].y + rv * ra[t].y) : 0.f;
-            da.z = m2 ? -lr * (c * rb[t].z + rv * ra[t].z) : 0.f;
-            da.w = m3 ? -lr * (c * rb[t].w + rv * ra[t].w) : 0.f;
-            db.x = m0 ? -lr * (c * ra[t].x + rv * rb[t].x) : 0.f;
-            db.y = m1 ? -lr * (c * ra[t].y + rv * rb[t].y) : 0.f;
-            db.z = m2 ? -lr * (c * ra[t].z + rv * rb[t].z) : 0.f;
-            db.w = m3 ? -lr * (c * ra[t].w + rv * rb[t].w) : 0.f;
-            if (!(fabsf(da.x) + fabsf(da.y) + fabsf(da.z) + fabsf(da.w) + fabsf(db.x) + fabsf(db.y) + fabsf(db.z) +
-                      fabsf(db.w) <= 3.0e38f))
-              bad = true;
-            fps_red_add4(pa[t], da);
-            fps_red_add4(pb[t], db);
-          }
-        }
-      }
-    }
-  }
-  if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
-  if (bad_id && a.bad_id != nullptr) *a.bad_id = 1;
-  if (a.predict_only) return;
-  fps_fm_bias_tail(a, loss_acc, lab_acc, g_acc);
-}
-
-template <typename IdT, int Q, int MINB, int TB, bool ONEHOT>
-__global__ void __launch_bounds__(FFM_THREADS, MINB) fps_ffm_adagrad_kernel(const __grid_constant__ FfmArgs a) {
-  constexpr int P = 32 / Q;        // pairs per warp per step
-  __shared__ FfmEntry s_ent[FFM_WARPS][2][FFM_CH];
-  __shared__ float* s_hrow[FFM_WARPS][2][FFM_CH];   // each staged entry's H row
-  const int lane = threadIdx.x & 31;
-  const int li = lane & (Q - 1);   // my float4 of the slab
-  const int gi = lane / Q;         // my lane-group
-  FfmEntry* entA = s_ent[threadIdx.x >> 5][0];
-  FfmEntry* entB = s_ent[threadIdx.x >> 5][1];
-  float** hA = s_hrow[threadIdx.x >> 5][0];
-  float** hB = s_hrow[threadIdx.x >> 5][1];
-  const int kp = 4 * ((a.k + 3) / 4);
-  // columns of my float4 inside the slab that hold factors: [k, kp) is padding and receives exact zeros; a lane
-  // whose float4 lies past the slab (kp / 4 < Q) neither pulls nor pushes
-  const int c0 = 4 * li;
-  const bool on = c0 < kp;
-  const bool m0 = c0 < a.k, m1 = c0 + 1 < a.k, m2 = c0 + 2 < a.k, m3 = c0 + 3 < a.k;
-  const float w0 = a.bias ? fps_ld_row4(fps_row(a.tab, a.num_features)).x : 0.f;
-
-  const long long warp = (blockIdx.x * (long long)FFM_THREADS + threadIdx.x) >> 5;
-  const long long n_warps = ((long long)gridDim.x * FFM_THREADS) >> 5;
-  float loss_acc = 0.f, lab_acc = 0.f;
-  double g_acc = 0.0;
-  bool bad = false, bad_id = false;
-
-  // one example per warp: the trip count is warp-uniform
-  for (long long ex = warp; ex < a.n; ex += n_warps) {
-    long long e = a.row_ptr[ex + 1];
-    long long b = a.row_ptr[ex];
-    if (e > a.nnz) e = a.nnz;
-    if (b < 0) b = 0;
-    if (b > e) b = e;
-    const int nc = (int)((e - b + FFM_CH - 1) / FFM_CH);
-    // ---- pass 1: linear term and pair terms --------------------------------------------------------------
-    float acc = 0.f, lin = 0.f;
-    for (int A = 0; A < nc; ++A) {
-      const int mA = ffm_stage<IdT, ONEHOT, 1>(a, entA, b + (long long)A * FFM_CH, e, 0.f, lin, bad, bad_id);
-      for (int B = A; B < nc; ++B) {
+    // ---- pass 2: re-pull both slabs of every pair (AdaGrad: with their H), push the deltas; dw as staged ----
+    if constexpr (ADA) {
+      float** hA = s_hrow[threadIdx.x >> 5][0];
+      float** hB = s_hrow[threadIdx.x >> 5][1];
+      for (int A = 0; A < nc; ++A) {
         float unused = 0.f;
-        const int mB = B == A ? mA : ffm_stage<IdT, ONEHOT, 0>(a, entB, b + (long long)B * FFM_CH, e, 0.f, unused,
-                                                               bad, bad_id);
-        const FfmEntry* eb = B == A ? entA : entB;
-        const int np = B == A ? mA * (mA - 1) / 2 : mA * mB;
-        for (int p0 = 0; p0 < np; p0 += P * TB) {
-          float4 ra[TB], rb[TB];
-          float xx[TB];
+        const int mA = ffm_stage<IdT, ONEHOT, 2, true>(a, entA, b + (long long)A * FFM_CH, e, g, unused, bad, bad_id,
+                                                        hA);
+        for (int B = A; B < nc; ++B) {
+          const int mB = B == A ? mA : ffm_stage<IdT, ONEHOT, 0, true>(a, entB, b + (long long)B * FFM_CH, e, 0.f,
+                                                                       unused, bad, bad_id, hB);
+          const FfmEntry* eb = B == A ? entA : entB;
+          float* const* hb_ = B == A ? hA : hB;
+          const int np = B == A ? mA * (mA - 1) / 2 : mA * mB;
+          for (int p0 = 0; p0 < np; p0 += P * TB) {
+            float4 ra[TB], rb[TB], ha[TB], hb[TB];
+            float* pa[TB];
+            float* pb[TB];
+            float* qa[TB];
+            float* qb[TB];
+            float cc[TB];
 #pragma unroll
-          for (int t = 0; t < TB; ++t) {
-            const int p = p0 + t * P + gi;
-            xx[t] = 0.f;
-            ra[t] = make_float4(0.f, 0.f, 0.f, 0.f);
-            rb[t] = ra[t];
-            if (p < np && on) {
-              int ia, ib;
-              ffm_pair(p, B == A, mB, ia, ib);
-              const FfmEntry ea = entA[ia], ebb = eb[ib];
-              xx[t] = ea.x * ebb.x;
-              ra[t] = fps_ld_row4(ea.row + 4 + ebb.field * kp + c0);   // V[i_a, f_b]
-              rb[t] = fps_ld_row4(ebb.row + 4 + ea.field * kp + c0);   // V[i_b, f_a]
+            for (int t = 0; t < TB; ++t) {
+              const int p = p0 + t * P + gi;
+              pa[t] = nullptr;
+              pb[t] = nullptr;
+              qa[t] = nullptr;
+              qb[t] = nullptr;
+              cc[t] = 0.f;
+              ra[t] = make_float4(0.f, 0.f, 0.f, 0.f);
+              rb[t] = ra[t];
+              ha[t] = ra[t];
+              hb[t] = ra[t];
+              if (p < np && on) {
+                int ia, ib;
+                ffm_pair(p, B == A, mB, ia, ib);
+                const FfmEntry ea = entA[ia], ebb = eb[ib];
+                cc[t] = g * (ea.x * ebb.x);
+                const int oa = 4 + ebb.field * kp + c0, ob = 4 + ea.field * kp + c0;
+                pa[t] = ea.row + oa;
+                pb[t] = ebb.row + ob;
+                qa[t] = hA[ia] + oa;
+                qb[t] = hb_[ib] + ob;
+                ra[t] = fps_ld_row4(pa[t]);
+                rb[t] = fps_ld_row4(pb[t]);
+                ha[t] = fps_ld_row4(qa[t]);
+                hb[t] = fps_ld_row4(qb[t]);
+              }
+            }
+#pragma unroll
+            for (int t = 0; t < TB; ++t) {
+              if (pa[t] == nullptr) continue;
+              const float c = cc[t], rv = a.reg_factors;
+              float4 ga, gb, gga, ggb;
+              ga.x = m0 ? c * rb[t].x + rv * ra[t].x : 0.f;
+              ga.y = m1 ? c * rb[t].y + rv * ra[t].y : 0.f;
+              ga.z = m2 ? c * rb[t].z + rv * ra[t].z : 0.f;
+              ga.w = m3 ? c * rb[t].w + rv * ra[t].w : 0.f;
+              gb.x = m0 ? c * ra[t].x + rv * rb[t].x : 0.f;
+              gb.y = m1 ? c * ra[t].y + rv * rb[t].y : 0.f;
+              gb.z = m2 ? c * ra[t].z + rv * rb[t].z : 0.f;
+              gb.w = m3 ? c * ra[t].w + rv * rb[t].w : 0.f;
+              const float4 da = fps_adagrad4(ga, ha[t], a.lr, gga);
+              const float4 db = fps_adagrad4(gb, hb[t], a.lr, ggb);
+              if (!(fabsf(da.x) + fabsf(da.y) + fabsf(da.z) + fabsf(da.w) + fabsf(db.x) + fabsf(db.y) + fabsf(db.z) +
+                        fabsf(db.w) + gga.x + gga.y + gga.z + gga.w + ggb.x + ggb.y + ggb.z + ggb.w <= 3.0e38f))
+                bad = true;
+              fps_red_add4(pa[t], da);
+              fps_red_add4(pb[t], db);
+              fps_red_add4(qa[t], gga);
+              fps_red_add4(qb[t], ggb);
             }
           }
-#pragma unroll
-          for (int t = 0; t < TB; ++t)
-            acc += xx[t] * (ra[t].x * rb[t].x + ra[t].y * rb[t].y + ra[t].z * rb[t].z + ra[t].w * rb[t].w);
         }
       }
-    }
-    const float yhat = w0 + fps_group_sum<32>(lin + acc);
-    if (lane == 0) a.pred[ex] = yhat;
-    if (a.predict_only) continue;
-    const float y = a.labels[ex];
-    if (y != y) continue;
-    float g;
-    if (a.loss == FFM_LOGISTIC) {
-      g = 1.f / (1.f + expf(-yhat)) - y;
-      if (lane == 0) loss_acc += fmaxf(yhat, 0.f) + log1pf(expf(-fabsf(yhat))) - y * yhat;
     } else {
-      g = yhat - y;
-      if (lane == 0) loss_acc += g * g;
-    }
-    if (lane == 0) {
-      lab_acc += 1.f;
-      g_acc += (double)g;
-    }
-    // ---- pass 2: re-pull both slabs of every pair with their H, push the deltas and gam^2; w as staged ------
-    for (int A = 0; A < nc; ++A) {
-      float unused = 0.f;
-      const int mA = ffm_stage<IdT, ONEHOT, 2, true>(a, entA, b + (long long)A * FFM_CH, e, g, unused, bad, bad_id,
-                                                      hA);
-      for (int B = A; B < nc; ++B) {
-        const int mB = B == A ? mA : ffm_stage<IdT, ONEHOT, 0, true>(a, entB, b + (long long)B * FFM_CH, e, 0.f,
-                                                                     unused, bad, bad_id, hB);
-        const FfmEntry* eb = B == A ? entA : entB;
-        float* const* hb_ = B == A ? hA : hB;
-        const int np = B == A ? mA * (mA - 1) / 2 : mA * mB;
-        for (int p0 = 0; p0 < np; p0 += P * TB) {
-          float4 ra[TB], rb[TB], ha[TB], hb[TB];
-          float* pa[TB];
-          float* pb[TB];
-          float* qa[TB];
-          float* qb[TB];
-          float cc[TB];
+      for (int A = 0; A < nc; ++A) {
+        float unused = 0.f;
+        const int mA = ffm_stage<IdT, ONEHOT, 2>(a, entA, b + (long long)A * FFM_CH, e, g, unused, bad, bad_id);
+        for (int B = A; B < nc; ++B) {
+          const int mB = B == A ? mA : ffm_stage<IdT, ONEHOT, 0>(a, entB, b + (long long)B * FFM_CH, e, 0.f, unused,
+                                                                 bad, bad_id);
+          const FfmEntry* eb = B == A ? entA : entB;
+          const int np = B == A ? mA * (mA - 1) / 2 : mA * mB;
+          for (int p0 = 0; p0 < np; p0 += P * TB) {
+            float4 ra[TB], rb[TB];
+            float* pa[TB];
+            float* pb[TB];
+            float cc[TB];
 #pragma unroll
-          for (int t = 0; t < TB; ++t) {
-            const int p = p0 + t * P + gi;
-            pa[t] = nullptr;
-            pb[t] = nullptr;
-            qa[t] = nullptr;
-            qb[t] = nullptr;
-            cc[t] = 0.f;
-            ra[t] = make_float4(0.f, 0.f, 0.f, 0.f);
-            rb[t] = ra[t];
-            ha[t] = ra[t];
-            hb[t] = ra[t];
-            if (p < np && on) {
-              int ia, ib;
-              ffm_pair(p, B == A, mB, ia, ib);
-              const FfmEntry ea = entA[ia], ebb = eb[ib];
-              cc[t] = g * (ea.x * ebb.x);
-              const int oa = 4 + ebb.field * kp + c0, ob = 4 + ea.field * kp + c0;
-              pa[t] = ea.row + oa;
-              pb[t] = ebb.row + ob;
-              qa[t] = hA[ia] + oa;
-              qb[t] = hb_[ib] + ob;
-              ra[t] = fps_ld_row4(pa[t]);
-              rb[t] = fps_ld_row4(pb[t]);
-              ha[t] = fps_ld_row4(qa[t]);
-              hb[t] = fps_ld_row4(qb[t]);
+            for (int t = 0; t < TB; ++t) {
+              const int p = p0 + t * P + gi;
+              pa[t] = nullptr;
+              pb[t] = nullptr;
+              cc[t] = 0.f;
+              ra[t] = make_float4(0.f, 0.f, 0.f, 0.f);
+              rb[t] = ra[t];
+              if (p < np && on) {
+                int ia, ib;
+                ffm_pair(p, B == A, mB, ia, ib);
+                const FfmEntry ea = entA[ia], ebb = eb[ib];
+                cc[t] = g * (ea.x * ebb.x);
+                pa[t] = ea.row + 4 + ebb.field * kp + c0;
+                pb[t] = ebb.row + 4 + ea.field * kp + c0;
+                ra[t] = fps_ld_row4(pa[t]);
+                rb[t] = fps_ld_row4(pb[t]);
+              }
             }
-          }
 #pragma unroll
-          for (int t = 0; t < TB; ++t) {
-            if (pa[t] == nullptr) continue;
-            const float c = cc[t], rv = a.reg_factors;
-            float4 ga, gb, gga, ggb;
-            ga.x = m0 ? c * rb[t].x + rv * ra[t].x : 0.f;
-            ga.y = m1 ? c * rb[t].y + rv * ra[t].y : 0.f;
-            ga.z = m2 ? c * rb[t].z + rv * ra[t].z : 0.f;
-            ga.w = m3 ? c * rb[t].w + rv * ra[t].w : 0.f;
-            gb.x = m0 ? c * ra[t].x + rv * rb[t].x : 0.f;
-            gb.y = m1 ? c * ra[t].y + rv * rb[t].y : 0.f;
-            gb.z = m2 ? c * ra[t].z + rv * rb[t].z : 0.f;
-            gb.w = m3 ? c * ra[t].w + rv * rb[t].w : 0.f;
-            const float4 da = fps_adagrad4(ga, ha[t], a.lr, gga);
-            const float4 db = fps_adagrad4(gb, hb[t], a.lr, ggb);
-            if (!(fabsf(da.x) + fabsf(da.y) + fabsf(da.z) + fabsf(da.w) + fabsf(db.x) + fabsf(db.y) + fabsf(db.z) +
-                      fabsf(db.w) + gga.x + gga.y + gga.z + gga.w + ggb.x + ggb.y + ggb.z + ggb.w <= 3.0e38f))
-              bad = true;
-            fps_red_add4(pa[t], da);
-            fps_red_add4(pb[t], db);
-            fps_red_add4(qa[t], gga);
-            fps_red_add4(qb[t], ggb);
+            for (int t = 0; t < TB; ++t) {
+              if (pa[t] == nullptr) continue;
+              const float c = cc[t], rv = a.reg_factors, lr = a.lr;
+              float4 da, db;
+              da.x = m0 ? -lr * (c * rb[t].x + rv * ra[t].x) : 0.f;
+              da.y = m1 ? -lr * (c * rb[t].y + rv * ra[t].y) : 0.f;
+              da.z = m2 ? -lr * (c * rb[t].z + rv * ra[t].z) : 0.f;
+              da.w = m3 ? -lr * (c * rb[t].w + rv * ra[t].w) : 0.f;
+              db.x = m0 ? -lr * (c * ra[t].x + rv * rb[t].x) : 0.f;
+              db.y = m1 ? -lr * (c * ra[t].y + rv * rb[t].y) : 0.f;
+              db.z = m2 ? -lr * (c * ra[t].z + rv * rb[t].z) : 0.f;
+              db.w = m3 ? -lr * (c * ra[t].w + rv * rb[t].w) : 0.f;
+              if (!(fabsf(da.x) + fabsf(da.y) + fabsf(da.z) + fabsf(da.w) + fabsf(db.x) + fabsf(db.y) + fabsf(db.z) +
+                        fabsf(db.w) <= 3.0e38f))
+                bad = true;
+              fps_red_add4(pa[t], da);
+              fps_red_add4(pb[t], db);
+            }
           }
         }
       }
     }
   }
-  if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
-  if (bad_id && a.bad_id != nullptr) *a.bad_id = 1;
-  if (a.predict_only) return;
-  fps_fm_bias_tail(a, loss_acc, lab_acc, g_acc);
+  fps_fm_bias_tail(a, bad, bad_id, loss_acc, lab_acc, g_acc);
 }
 
 template <typename IdT, int Q, int MINB, int TB, bool ADA>
 static int launch_ffm(const FfmArgs& a, int num_sms, cudaStream_t stream) {
-  void (*kern)(const FfmArgs);
-  if constexpr (ADA)
-    kern = a.vals == nullptr ? fps_ffm_adagrad_kernel<IdT, Q, MINB, TB, true>
-                             : fps_ffm_adagrad_kernel<IdT, Q, MINB, TB, false>;
-  else
-    kern = a.vals == nullptr ? fps_ffm_kernel<IdT, Q, MINB, TB, true> : fps_ffm_kernel<IdT, Q, MINB, TB, false>;
+  void (*kern)(const FfmArgs) = a.vals == nullptr ? fps_ffm_kernel<IdT, Q, MINB, TB, true, ADA>
+                                                  : fps_ffm_kernel<IdT, Q, MINB, TB, false, ADA>;
   long long blocks = fps_row_grid(kern, FFM_THREADS, FFM_WARPS, num_sms, a.reserve_total, 0, 1, a.n, 1);
   if (a.max_ctas > 0 && blocks > a.max_ctas) blocks = a.max_ctas;
   kern<<<(int)blocks, FFM_THREADS, 0, stream>>>(a);
@@ -482,7 +388,7 @@ extern "C" int fps_ffm_step(const FfmArgs* args, int id_bytes, int num_sms, cuda
   const FfmArgs& a = *args;
   if (a.k < 1 || a.k > FFM_MAX_K || a.num_fields < 1 || a.num_fields > FFM_MAX_FIELDS) return -1702;
   if (a.tab.stride != 4 + a.num_fields * 4 * ((a.k + 3) / 4) || a.tab.dim != a.tab.stride) return -1701;
-  if (a.loss != FFM_LOGISTIC && a.loss != FFM_SQUARED) return -1703;
+  if (a.loss != FM_LOGISTIC && a.loss != FM_SQUARED) return -1703;
   if (a.n < 0 || a.n >= INT_MAX || a.nnz < 0 || a.num_features < 0) return -1704;
   if (a.bias && !a.predict_only && (a.bias_acc == nullptr || a.bias_done == nullptr)) return -1705;
   const bool ada = a.acc.base[0] != nullptr;

@@ -17,10 +17,12 @@
 // outside [0, num_features) are skipped and raise *bad_id; the end of every example is clamped to nnz.
 //
 // AdaGrad (DESIGN §2.17, libffm's element-wise rule): with acc.base[0] set, acc is a second table of the same
-// geometry holding H = G - 1 per element (a zero heap is the starting state).  For every element the SGD rule would
-// step by -lr * gam (gam = the bracket above), fps_fm_adagrad_kernel pulls H with the row chunk and pushes
+// geometry holding H = G - 1 per element (a zero heap is the starting state), and the step launches fps_fm_kernel
+// with ADA set.  Everything up to g is shared; only pass 2 differs: for every element the SGD rule would step by
+// -lr * gam (gam = the bracket above), fm_push_adagrad pulls H with the row chunk and pushes
 //   dtheta = -lr * gam / sqrtf(1 + H + gam^2)   and   dH = gam^2
-// with two red.add.v4.f32 (padding: gam = 0, so both stay exactly zero).  w0 keeps the SGD rule.
+// with two red.add.v4.f32 (padding: gam = 0, so both stay exactly zero).  w0 keeps the SGD rule.  The two pass 2
+// bodies stay apart: one body with the H loads under if constexpr changes the SGD instantiations' code.
 #include <limits.h>
 #include "fps_common.cuh"
 #include "fps_fm_bias.cuh"
@@ -28,7 +30,6 @@
 
 #define FM_THREADS 256
 #define FM_BIT(c, i) ((fbits >> (4 * (c) + (i))) & 1u)
-enum FmLoss : int { FM_LOGISTIC = 0, FM_SQUARED = 1 };
 
 struct FmArgs {
   const long long* row_ptr;  // [n + 1]
@@ -59,7 +60,7 @@ struct FmArgs {
 };
 
 // AdaGrad pass 2 of one example (entries [b, e), gradient g, s = sum x v): re-pull each row chunk with its H chunk,
-// push dtheta and gam^2.  fbits as in fm_body.
+// push dtheta and gam^2.  fbits as in fps_fm_kernel.
 template <typename IdT, int LPR, int VPL, int TB, bool ONEHOT>
 __device__ __forceinline__ void fm_push_adagrad(const FmArgs& a, long long b, long long e, float g,
                                                 const float4 (&s)[VPL], unsigned fbits, bool& bad) {
@@ -119,7 +120,7 @@ __device__ __forceinline__ void fm_push_adagrad(const FmArgs& a, long long b, lo
   }
 }
 
-template <typename IdT, int LPR, int VPL, int MINB, int TB, bool ONEHOT>
+template <typename IdT, int LPR, int VPL, int MINB, int TB, bool ONEHOT, bool ADA>
 __global__ void __launch_bounds__(FM_THREADS, MINB) fps_fm_kernel(const __grid_constant__ FmArgs a) {
   constexpr int GPW = 32 / LPR;   // examples per warp per round
   const IdT* __restrict__ cols = reinterpret_cast<const IdT*>(a.cols);
@@ -218,175 +219,61 @@ __global__ void __launch_bounds__(FM_THREADS, MINB) fps_fm_kernel(const __grid_c
       lab_acc += 1.f;
       g_acc += (double)g;
     }
-    // ---- pass 2: re-pull, delta, push -------------------------------------------------------------------
-    for (long long j0 = b; j0 < e; j0 += TB) {
-      float x[TB];
-      float* rp[TB];
-      float4 r[TB][VPL];
-#pragma unroll
-      for (int t = 0; t < TB; ++t) {
-        const long long j = j0 + t;
-        rp[t] = nullptr;
-        x[t] = 0.f;
-        if (j < e) {
-          const long long id = (long long)cols[j];
-          if (id >= 0 && id < a.num_features) {
-            rp[t] = fps_row_t<IdT>(a.tab, (IdT)id);
-            x[t] = ONEHOT ? 1.f : a.vals[j];
-          }
-        }
-#pragma unroll
-        for (int c = 0; c < VPL; ++c) {
-          const int q = lane + c * LPR;
-          r[t][c] = (rp[t] != nullptr && q < nvec) ? fps_ld_row4(rp[t] + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-#pragma unroll
-      for (int t = 0; t < TB; ++t) {
-        if (rp[t] == nullptr) continue;
-        const float gx = g * x[t];
-#pragma unroll
-        for (int c = 0; c < VPL; ++c) {
-          const int q = lane + c * LPR;
-          if (q >= nvec) continue;
-          const float4 v = r[t][c];
-          float4 d;
-          d.x = FM_BIT(c, 0) ? -a.lr * (gx * (s[c].x - x[t] * v.x) + a.reg_factors * v.x) : 0.f;
-          d.y = FM_BIT(c, 1) ? -a.lr * (gx * (s[c].y - x[t] * v.y) + a.reg_factors * v.y) : 0.f;
-          d.z = FM_BIT(c, 2) ? -a.lr * (gx * (s[c].z - x[t] * v.z) + a.reg_factors * v.z) : 0.f;
-          d.w = FM_BIT(c, 3) ? -a.lr * (gx * (s[c].w - x[t] * v.w) + a.reg_factors * v.w) : 0.f;
-          if (c == 0 && has_w) d.x = -a.lr * (gx + a.reg_linear * v.x);
-          if (!(fabsf(d.x) + fabsf(d.y) + fabsf(d.z) + fabsf(d.w) <= 3.0e38f)) bad = true;
-          fps_red_add4(rp[t] + 4 * q, d);   // the PUSH fused with paramUpdate (+)
-        }
-      }
-    }
-  }
-  if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
-  if (bad_id && a.bad_id != nullptr) *a.bad_id = 1;
-  if (a.predict_only) return;
-  fps_fm_bias_tail(a, loss_acc, lab_acc, g_acc);   // per-warp sums; the last CTA steps w0
-}
-
-// AdaGrad twin of fps_fm_kernel: the same pass 1, pass 2 through fm_push_adagrad.  A separate body, so the SGD
-// kernel's code is untouched.
-template <typename IdT, int LPR, int VPL, int MINB, int TB, bool ONEHOT>
-__global__ void __launch_bounds__(FM_THREADS, MINB) fps_fm_adagrad_kernel(const __grid_constant__ FmArgs a) {
-  constexpr int GPW = 32 / LPR;   // examples per warp per round
-  const IdT* __restrict__ cols = reinterpret_cast<const IdT*>(a.cols);
-  const int lane = threadIdx.x & (LPR - 1);
-  const int nvec = a.tab.stride >> 2;
-  const int dim = a.dim;
-  // factor columns of my chunks: bit 4c + i is set iff column 4 (lane + c LPR) + i lies in [1, dim)
-  unsigned fbits = 0u;
-#pragma unroll
-  for (int c = 0; c < VPL; ++c)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int col = 4 * (lane + c * LPR) + i;
-      if (col >= 1 && col < dim) fbits |= 1u << (4 * c + i);
-    }
-  const bool has_w = lane == 0;   // chunk 0, column 0 of every row is w
-  const float w0 = a.bias ? fps_ld_row4(fps_row(a.tab, a.num_features)).x : 0.f;
-
-  const long long warp = (blockIdx.x * (long long)FM_THREADS + threadIdx.x) >> 5;
-  const long long n_warps = ((long long)gridDim.x * FM_THREADS) >> 5;
-  const int grp = (threadIdx.x & 31) / LPR;
-  float loss_acc = 0.f, lab_acc = 0.f;
-  double g_acc = 0.0;
-  bool bad = false, bad_id = false;
-
-  // warp-uniform trip count: every lane reaches the group sums of every round
-  for (long long base = warp * GPW; base < a.n; base += n_warps * GPW) {
-    const long long ex = base + grp;
-    const bool live = ex < a.n;
-    long long b = 0, e = 0;
-    if (live) {
-      e = a.row_ptr[ex + 1];
-      b = a.row_ptr[ex];
-      if (e > a.nnz) e = a.nnz;
-      if (b < 0) b = 0;
-      if (b > e) b = e;
-    }
-    // ---- pass 1: linear term, s, sum x^2 v^2 ------------------------------------------------------------
-    float4 s[VPL];
-#pragma unroll
-    for (int c = 0; c < VPL; ++c) s[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-    float lin = 0.f, sq = 0.f;
-    for (long long j0 = b; j0 < e; j0 += TB) {
-      float x[TB];
-      float4 r[TB][VPL];
-#pragma unroll
-      for (int t = 0; t < TB; ++t) {
-        const long long j = j0 + t;
-        x[t] = 0.f;
-        const float* row = nullptr;
-        if (j < e) {
-          const long long id = (long long)cols[j];
-          if (id >= 0 && id < a.num_features) {
-            row = fps_row_t<IdT>(a.tab, (IdT)id);
-            x[t] = ONEHOT ? 1.f : a.vals[j];
-          } else {
-            bad_id = true;
-          }
-        }
-#pragma unroll
-        for (int c = 0; c < VPL; ++c) {
-          const int q = lane + c * LPR;
-          r[t][c] = (row != nullptr && q < nvec) ? fps_ld_row4(row + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-#pragma unroll
-      for (int t = 0; t < TB; ++t) {
-        if (has_w) lin += x[t] * r[t][0].x;
-#pragma unroll
-        for (int c = 0; c < VPL; ++c) {
-          const float4 v = make_float4(FM_BIT(c, 0) ? x[t] * r[t][c].x : 0.f, FM_BIT(c, 1) ? x[t] * r[t][c].y : 0.f,
-                                       FM_BIT(c, 2) ? x[t] * r[t][c].z : 0.f, FM_BIT(c, 3) ? x[t] * r[t][c].w : 0.f);
-          s[c].x += v.x; s[c].y += v.y; s[c].z += v.z; s[c].w += v.w;
-          sq += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
-        }
-      }
-    }
-    float ss = 0.f;
-#pragma unroll
-    for (int c = 0; c < VPL; ++c) ss += s[c].x * s[c].x + s[c].y * s[c].y + s[c].z * s[c].z + s[c].w * s[c].w;
-    const float yhat = w0 + fps_group_sum<LPR>(lin + 0.5f * (ss - sq));
-    if (!live) continue;
-    if (lane == 0) a.pred[ex] = yhat;
-    if (a.predict_only) continue;
-    const float y = a.labels[ex];
-    if (y != y) continue;
-    float g;
-    if (a.loss == FM_LOGISTIC) {
-      g = 1.f / (1.f + expf(-yhat)) - y;
-      if (lane == 0) loss_acc += fmaxf(yhat, 0.f) + log1pf(expf(-fabsf(yhat))) - y * yhat;
+    // ---- pass 2: re-pull (with H under AdaGrad), delta, push ----------------------------------------------
+    if constexpr (ADA) {
+      fm_push_adagrad<IdT, LPR, VPL, TB, ONEHOT>(a, b, e, g, s, fbits, bad);
     } else {
-      g = yhat - y;
-      if (lane == 0) loss_acc += g * g;
+      for (long long j0 = b; j0 < e; j0 += TB) {
+        float x[TB];
+        float* rp[TB];
+        float4 r[TB][VPL];
+#pragma unroll
+        for (int t = 0; t < TB; ++t) {
+          const long long j = j0 + t;
+          rp[t] = nullptr;
+          x[t] = 0.f;
+          if (j < e) {
+            const long long id = (long long)cols[j];
+            if (id >= 0 && id < a.num_features) {
+              rp[t] = fps_row_t<IdT>(a.tab, (IdT)id);
+              x[t] = ONEHOT ? 1.f : a.vals[j];
+            }
+          }
+#pragma unroll
+          for (int c = 0; c < VPL; ++c) {
+            const int q = lane + c * LPR;
+            r[t][c] = (rp[t] != nullptr && q < nvec) ? fps_ld_row4(rp[t] + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
+          }
+        }
+#pragma unroll
+        for (int t = 0; t < TB; ++t) {
+          if (rp[t] == nullptr) continue;
+          const float gx = g * x[t];
+#pragma unroll
+          for (int c = 0; c < VPL; ++c) {
+            const int q = lane + c * LPR;
+            if (q >= nvec) continue;
+            const float4 v = r[t][c];
+            float4 d;
+            d.x = FM_BIT(c, 0) ? -a.lr * (gx * (s[c].x - x[t] * v.x) + a.reg_factors * v.x) : 0.f;
+            d.y = FM_BIT(c, 1) ? -a.lr * (gx * (s[c].y - x[t] * v.y) + a.reg_factors * v.y) : 0.f;
+            d.z = FM_BIT(c, 2) ? -a.lr * (gx * (s[c].z - x[t] * v.z) + a.reg_factors * v.z) : 0.f;
+            d.w = FM_BIT(c, 3) ? -a.lr * (gx * (s[c].w - x[t] * v.w) + a.reg_factors * v.w) : 0.f;
+            if (c == 0 && has_w) d.x = -a.lr * (gx + a.reg_linear * v.x);
+            if (!(fabsf(d.x) + fabsf(d.y) + fabsf(d.z) + fabsf(d.w) <= 3.0e38f)) bad = true;
+            fps_red_add4(rp[t] + 4 * q, d);   // the PUSH fused with paramUpdate (+)
+          }
+        }
+      }
     }
-    if (lane == 0) {
-      lab_acc += 1.f;
-      g_acc += (double)g;
-    }
-    // ---- pass 2: re-pull with H, delta, push both -------------------------------------------------------
-    fm_push_adagrad<IdT, LPR, VPL, TB, ONEHOT>(a, b, e, g, s, fbits, bad);
   }
-  if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
-  if (bad_id && a.bad_id != nullptr) *a.bad_id = 1;
-  if (a.predict_only) return;
-  fps_fm_bias_tail(a, loss_acc, lab_acc, g_acc);   // per-warp sums; the last CTA steps w0
+  fps_fm_bias_tail(a, bad, bad_id, loss_acc, lab_acc, g_acc);   // per-warp sums; the last CTA steps w0
 }
 
 template <typename IdT, int LPR, int VPL, int MINB, int TB, bool ADA>
 static int launch_fm(const FmArgs& a, int num_sms, cudaStream_t stream) {
-  void (*kern)(const FmArgs);
-  if constexpr (ADA)
-    kern = a.vals == nullptr ? fps_fm_adagrad_kernel<IdT, LPR, VPL, MINB, TB, true>
-                             : fps_fm_adagrad_kernel<IdT, LPR, VPL, MINB, TB, false>;
-  else
-    kern = a.vals == nullptr ? fps_fm_kernel<IdT, LPR, VPL, MINB, TB, true>
-                             : fps_fm_kernel<IdT, LPR, VPL, MINB, TB, false>;
+  void (*kern)(const FmArgs) = a.vals == nullptr ? fps_fm_kernel<IdT, LPR, VPL, MINB, TB, true, ADA>
+                                                 : fps_fm_kernel<IdT, LPR, VPL, MINB, TB, false, ADA>;
   long long blocks = fps_row_grid(kern, FM_THREADS, FM_THREADS / LPR, num_sms, a.reserve_total, 0, 1, a.n, 1);
   if (a.max_ctas > 0 && blocks > a.max_ctas) blocks = a.max_ctas;
   kern<<<(int)blocks, FM_THREADS, 0, stream>>>(a);
@@ -394,37 +281,22 @@ static int launch_fm(const FmArgs& a, int num_sms, cudaStream_t stream) {
 }
 
 // Lane geometry of w2v_dispatch: LPR = nvec up to 32 float4, then 32 lanes with VPL = 2, 3 or 4; MINB keeps every
-// instantiation free of spills (ptxas -v, DESIGN §3).
-template <typename IdT>
+// instantiation free of spills (ptxas -v, DESIGN §3).  Under AdaGrad the H chunks double r[TB][VPL], so the narrow
+// rungs pull 4 rows at a time instead of 8.
+template <typename IdT, bool ADA>
 static int fm_dispatch(const FmArgs& a, int num_sms, cudaStream_t s) {
+  constexpr int TB = ADA ? 4 : 8;
   const int nvec = a.tab.stride >> 2;
-  if (nvec <= 1) return launch_fm<IdT, 1, 1, 2, 8, false>(a, num_sms, s);
-  if (nvec <= 2) return launch_fm<IdT, 2, 1, 2, 8, false>(a, num_sms, s);
-  if (nvec <= 4) return launch_fm<IdT, 4, 1, 2, 8, false>(a, num_sms, s);
-  if (nvec <= 8) return launch_fm<IdT, 8, 1, 2, 8, false>(a, num_sms, s);
-  if (nvec <= 16) return launch_fm<IdT, 16, 1, 2, 8, false>(a, num_sms, s);
-  if (nvec <= 32) return launch_fm<IdT, 32, 1, 2, 8, false>(a, num_sms, s);
-  if (nvec <= 64) return launch_fm<IdT, 32, 2, 1, 4, false>(a, num_sms, s);
-  if (nvec <= 96) return launch_fm<IdT, 32, 3, 1, 4, false>(a, num_sms, s);
-  if (nvec <= 128) return launch_fm<IdT, 32, 4, 1, 4, false>(a, num_sms, s);
+  if (nvec <= 1) return launch_fm<IdT, 1, 1, 2, TB, ADA>(a, num_sms, s);
+  if (nvec <= 2) return launch_fm<IdT, 2, 1, 2, TB, ADA>(a, num_sms, s);
+  if (nvec <= 4) return launch_fm<IdT, 4, 1, 2, TB, ADA>(a, num_sms, s);
+  if (nvec <= 8) return launch_fm<IdT, 8, 1, 2, TB, ADA>(a, num_sms, s);
+  if (nvec <= 16) return launch_fm<IdT, 16, 1, 2, TB, ADA>(a, num_sms, s);
+  if (nvec <= 32) return launch_fm<IdT, 32, 1, 2, TB, ADA>(a, num_sms, s);
+  if (nvec <= 64) return launch_fm<IdT, 32, 2, 1, 4, ADA>(a, num_sms, s);
+  if (nvec <= 96) return launch_fm<IdT, 32, 3, 1, 4, ADA>(a, num_sms, s);
+  if (nvec <= 128) return launch_fm<IdT, 32, 4, 1, 4, ADA>(a, num_sms, s);
   return -1000;   // rows wider than 512 floats
-}
-
-// The same lane ladder for AdaGrad; the H chunks double r[TB][VPL], so the wide rungs pull fewer rows at a time
-// (no spills, DESIGN §3).
-template <typename IdT>
-static int fm_adagrad_dispatch(const FmArgs& a, int num_sms, cudaStream_t s) {
-  const int nvec = a.tab.stride >> 2;
-  if (nvec <= 1) return launch_fm<IdT, 1, 1, 2, 4, true>(a, num_sms, s);
-  if (nvec <= 2) return launch_fm<IdT, 2, 1, 2, 4, true>(a, num_sms, s);
-  if (nvec <= 4) return launch_fm<IdT, 4, 1, 2, 4, true>(a, num_sms, s);
-  if (nvec <= 8) return launch_fm<IdT, 8, 1, 2, 4, true>(a, num_sms, s);
-  if (nvec <= 16) return launch_fm<IdT, 16, 1, 2, 4, true>(a, num_sms, s);
-  if (nvec <= 32) return launch_fm<IdT, 32, 1, 2, 4, true>(a, num_sms, s);
-  if (nvec <= 64) return launch_fm<IdT, 32, 2, 1, 4, true>(a, num_sms, s);
-  if (nvec <= 96) return launch_fm<IdT, 32, 3, 1, 4, true>(a, num_sms, s);
-  if (nvec <= 128) return launch_fm<IdT, 32, 4, 1, 4, true>(a, num_sms, s);
-  return -1000;
 }
 
 extern "C" int fps_fm_step(const FmArgs* args, int id_bytes, int num_sms, cudaStream_t stream) {
@@ -439,12 +311,9 @@ extern "C" int fps_fm_step(const FmArgs* args, int id_bytes, int num_sms, cudaSt
   if (a.n == 0) return 0;
   // predictions come from the AdaGrad kernel too (its pass 1 sums in the same blocks as its training step); with
   // predict_only it never reaches H
-  if (ada) {
-    if (id_bytes == 4) return fm_adagrad_dispatch<int>(a, num_sms, stream);
-    if (id_bytes == 8) return fm_adagrad_dispatch<long long>(a, num_sms, stream);
-    return -1001;
-  }
-  if (id_bytes == 4) return fm_dispatch<int>(a, num_sms, stream);
-  if (id_bytes == 8) return fm_dispatch<long long>(a, num_sms, stream);
+  if (id_bytes == 4)
+    return ada ? fm_dispatch<int, true>(a, num_sms, stream) : fm_dispatch<int, false>(a, num_sms, stream);
+  if (id_bytes == 8)
+    return ada ? fm_dispatch<long long, true>(a, num_sms, stream) : fm_dispatch<long long, false>(a, num_sms, stream);
   return -1001;
 }

@@ -1,9 +1,11 @@
-// The end of a factorization-machine launch, shared by fps_fm.cu and fps_ffm.cu (DESIGN §2.15, §2.16): per-warp
-// sums of the loss, the labelled count and sum g into `stats` and `bias_acc`, then the w0 rule.  Every example reads
-// w0 as it was before the launch; the last CTA to finish (a launch counter that resets itself, behind
+// What fps_fm.cu and fps_ffm.cu share (DESIGN §2.15, §2.16): the losses and the end of a launch: the error flags,
+// per-warp sums of the loss, the labelled count and sum g into `stats` and `bias_acc`, then the w0 rule.  Every
+// example reads w0 as it was before the launch; the last CTA to finish (a launch counter that resets itself, behind
 // __threadfence) pushes -lr * sum g / n_labelled to column 0 of the bias row, once per launch.
 #pragma once
 #include "fps_common.cuh"
+
+enum FmLoss : int { FM_LOGISTIC = 0, FM_SQUARED = 1 };
 
 __device__ __forceinline__ void fps_red_add1(float* p, float v) {
   asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
@@ -27,10 +29,15 @@ __device__ __forceinline__ float4 fps_adagrad4(float4 gam, float4 h, float lr, f
                      fps_adagrad1(gam.z, h.z, lr, gg.z), fps_adagrad1(gam.w, h.w, lr, gg.w));
 }
 
-// Args: FmArgs or FfmArgs (stats, bias, bias_acc, bias_done, lr, nan_flag, tab, num_features).  Every thread of the
-// CTA calls it after its last example; loss_acc, lab_acc and g_acc are the thread's own sums.
+// Args: FmArgs or FfmArgs (nan_flag, bad_id, predict_only, stats, bias, bias_acc, bias_done, lr, tab,
+// num_features).  Every thread of the CTA calls it after its last example: bad and bad_id raise the flags, and
+// unless the launch only predicts, loss_acc, lab_acc and g_acc (the thread's own sums) go on to the w0 rule.
 template <typename Args>
-__device__ __forceinline__ void fps_fm_bias_tail(const Args& a, float loss_acc, float lab_acc, double g_acc) {
+__device__ __forceinline__ void fps_fm_bias_tail(const Args& a, bool bad, bool bad_id, float loss_acc, float lab_acc,
+                                                 double g_acc) {
+  if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
+  if (bad_id && a.bad_id != nullptr) *a.bad_id = 1;
+  if (a.predict_only) return;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, o);

@@ -20,10 +20,17 @@ at most ``N EPS sum|terms|``; ``yhat`` counts every pair and entry of the exampl
 softplus add ``4 EPS``; each product, difference and push adds one rounding of its magnitude.  ``breaks`` switches one
 rule off (the sensitivity checks of the GPU suite): ``"field_unaware"`` pairs ``V[i_a, f_a]`` with ``V[i_b, f_b]``,
 ``"self_pairs"`` takes ``a <= b``, ``"no_xx"`` drops ``x_a x_b`` from the slab deltas, ``"w0_per_example"`` steps
-``w0`` after every example, ``"reg_sign"`` flips the regularisation's sign in the deltas."""
+``w0`` after every example, ``"reg_sign"`` flips the regularisation's sign in the deltas.
+
+AdaGrad (DESIGN §2.17): ``acc`` / ``acc_tol`` are ``H`` and its bounds, as in tests/fm_ref.py, whose rule, error
+model and ``ADAGRAD_BREAKS`` apply to ``w`` and to both slabs of every pair; ``acc=None`` is plain SGD.  ``stale``
+and ``repull`` apply to ``H`` as to the slabs: a slab pushed twice inside one example reads an ``H`` that may or may
+not hold the earlier pair's ``gam^2`` (PTX orders a reduction only before the same thread's own later loads)."""
 import math
 
 import numpy as np
+
+from tests.fm_ref import ADAGRAD_BREAKS, adagrad
 
 EPS = 2.0 ** -24
 MARGIN = 2.0
@@ -59,17 +66,24 @@ def _slab_cols(f, k, kp):
 
 def replay(table, row_ptr, cols, fields, vals, labels, *, num_features, num_fields, k, loss="logistic", lr=0.05,
            reg_linear=0.0, reg_factors=0.0, bias=True, predict_only=False, tol=None, fp32=True, breaks=None,
-           stale=False, repull=False):
+           stale=False, repull=False, acc=None, acc_tol=None):
     """Replay one launch.  ``table`` ``[num_features + 1, stride]``: the rows as the kernel reads them (float64
     copies of the fp32 table; ``tol`` their bounds, default 0).  Returns a :class:`Result` with ``table`` and
     ``tol`` after the launch, ``pred`` / ``tol_pred``, ``g``, ``loss_sum``, ``labelled``, ``w0_delta`` and
     ``bad_id``.  ``repull=True`` computes every push of an example from the rows as its earlier pushes left them
-    (the kernel's pass 2 re-pulls; with a slab pushed twice in one example it lies between the two ends)."""
-    if breaks is not None and breaks not in BREAKS:
+    (the kernel's pass 2 re-pulls; with a slab pushed twice in one example it lies between the two ends).  ``acc``
+    / ``acc_tol``: AdaGrad's ``H`` and its bounds, as in tests/fm_ref.py; the result's ``acc`` / ``tol_acc`` are
+    ``None`` without them."""
+    if breaks is not None and breaks not in BREAKS + (ADAGRAD_BREAKS if acc is not None else ()):
         raise ValueError(f"unknown break {breaks!r}")
     W = np.array(table, dtype=np.float64)
     T = np.zeros_like(W) if tol is None else np.array(tol, dtype=np.float64)
     R, RT = (W.copy(), T.copy()) if stale else (W, T)   # the rows each example reads
+    ada = acc is not None
+    if ada:
+        Hm = np.array(acc, dtype=np.float64)
+        TH = np.zeros_like(Hm) if acc_tol is None else np.array(acc_tol, dtype=np.float64)
+        RH, RTH = (Hm.copy(), TH.copy()) if stale else (Hm, TH)
     nf, F, k = int(num_features), int(num_fields), int(k)
     kp = kpad(k)
     if W.shape[1] != stride(F, k):
@@ -153,40 +167,63 @@ def replay(table, row_ptr, cols, fields, vals, labels, *, num_features, num_fiel
             scol = np.concatenate([ca, cb])
             D, TD = np.concatenate([dA, dB]), np.concatenate([tdA, tdB])
             keys = rows * (F + 1) + (scol[:, 0] - 4) // kp if len(rows) else rows
+            if ada:
+                # the brackets without -lr, each with H as the example pulled it
+                gw = gx + rl * w
+                tgw = np.abs(x) * tg + abs(rl) * tw + 2 * EPS * (np.abs(gx) + np.abs(rl * w))
+                dw, tdw, dHw, tdHw = adagrad(gw, tgw, RH[idx, 0], RTH[idx, 0], lr, breaks, gx)
+                gA, gB = c[:, None] * VB + rv * VA, c[:, None] * VA + rv * VB
+                tgA = (tc[:, None] * np.abs(VB) + np.abs(c)[:, None] * tVB + abs(rv) * tVA
+                       + 2 * EPS * (np.abs(c[:, None] * VB) + np.abs(rv * VA)))
+                tgB = (tc[:, None] * np.abs(VA) + np.abs(c)[:, None] * tVA + abs(rv) * tVB
+                       + 2 * EPS * (np.abs(c[:, None] * VA) + np.abs(rv * VB)))
+                G_, TG = np.concatenate([gA, gB]), np.concatenate([tgA, tgB])
+                GL = np.concatenate([c[:, None] * VB, c[:, None] * VA])
+                D, TD, DH, TDH = adagrad(G_, TG, RH[rows[:, None], scol], RTH[rows[:, None], scol], lr, breaks, GL)
+
+            def push(Wt, Tt, i, cc, d, td):
+                new = ftz(Wt[i, cc] + ftz(d))
+                Tt[i, cc] = Tt[i, cc] + td + EPS * np.abs(new)
+                Wt[i, cc] = new
+
             if repull:
-                # the other end of the race inside the example: each entry and pair reads its rows as the pushes
-                # before it left them
+                # the other end of the race inside the example: each entry and pair reads its rows (and H) as the
+                # pushes before it left them
                 for j in range(m):
                     i = int(idx[j])
-                    d = -lr * (gx[j] + rl * W[i, 0])
-                    new = float(ftz(W[i, 0] + ftz(d)))
-                    T[i, 0] = T[i, 0] + tdw[j] + EPS * abs(new)
-                    W[i, 0] = new
+                    if ada:
+                        d, td, dh, tdh = adagrad(gx[j] + rl * W[i, 0], tgw[j], Hm[i, 0], TH[i, 0], lr, breaks, gx[j])
+                        push(W, T, i, 0, float(d), float(td))
+                        push(Hm, TH, i, 0, float(dh), float(tdh))
+                    else:
+                        push(W, T, i, 0, -lr * (gx[j] + rl * W[i, 0]), tdw[j])
                 for j in range(len(pa)):
                     va, vb = W[ra[j], ca[j]], W[rb[j], cb[j]]
-                    for i, cc, d, td in ((ra[j], ca[j], -lr * (c[j] * vb + rv * va), tdA[j]),
-                                         (rb[j], cb[j], -lr * (c[j] * va + rv * vb), tdB[j])):
-                        new = ftz(W[i, cc] + ftz(d))
-                        T[i, cc] = T[i, cc] + td + EPS * np.abs(new)
-                        W[i, cc] = new
+                    if ada:
+                        for i, cc, gm, tgm, gl in ((ra[j], ca[j], c[j] * vb + rv * va, tgA[j], c[j] * vb),
+                                                   (rb[j], cb[j], c[j] * va + rv * vb, tgB[j], c[j] * va)):
+                            d, td, dh, tdh = adagrad(gm, tgm, Hm[i, cc], TH[i, cc], lr, breaks, gl)
+                            push(W, T, i, cc, d, td)
+                            push(Hm, TH, i, cc, dh, tdh)
+                    else:
+                        for i, cc, d, td in ((ra[j], ca[j], -lr * (c[j] * vb + rv * va), tdA[j]),
+                                             (rb[j], cb[j], -lr * (c[j] * va + rv * vb), tdB[j])):
+                            push(W, T, i, cc, d, td)
             elif len(np.unique(idx)) == m and len(np.unique(keys)) == len(keys):
-                new = ftz(W[idx, 0] + ftz(dw))
-                T[idx, 0] = T[idx, 0] + tdw + EPS * np.abs(new)
-                W[idx, 0] = new
-                new = ftz(W[rows[:, None], scol] + ftz(D))
-                T[rows[:, None], scol] = T[rows[:, None], scol] + TD + EPS * np.abs(new)
-                W[rows[:, None], scol] = new
+                push(W, T, idx, 0, dw, tdw)
+                push(W, T, rows[:, None], scol, D, TD)
+                if ada:
+                    push(Hm, TH, idx, 0, dHw, tdHw)
+                    push(Hm, TH, rows[:, None], scol, DH, TDH)
             else:
                 for j in range(m):   # a repeated feature or slab: its pushes land one after the other
-                    i = int(idx[j])
-                    new = float(ftz(W[i, 0] + ftz(dw[j])))
-                    T[i, 0] = T[i, 0] + tdw[j] + EPS * abs(new)
-                    W[i, 0] = new
+                    push(W, T, int(idx[j]), 0, dw[j], tdw[j])
+                    if ada:
+                        push(Hm, TH, int(idx[j]), 0, dHw[j], tdHw[j])
                 for j in range(len(rows)):
-                    i, cc = int(rows[j]), scol[j]
-                    new = ftz(W[i, cc] + ftz(D[j]))
-                    T[i, cc] = T[i, cc] + TD[j] + EPS * np.abs(new)
-                    W[i, cc] = new
+                    push(W, T, int(rows[j]), scol[j], D[j], TD[j])
+                    if ada:
+                        push(Hm, TH, int(rows[j]), scol[j], DH[j], TDH[j])
             if breaks == "w0_per_example" and bias:
                 w0 = float(ftz(w0 + ftz(-lr * g)))
                 tw0 = tw0 + lr * tg + 2 * EPS * abs(w0)
@@ -202,8 +239,10 @@ def replay(table, row_ptr, cols, fields, vals, labels, *, num_features, num_fiel
             T[nf, 0] = T[nf, 0] + lr * sum_tg / labelled + 2 * EPS * abs(w0_delta) + EPS * abs(new)
             W[nf, 0] = new
     T = np.where(np.isfinite(T), T, 0.0)
+    if ada:
+        TH = np.where(np.isfinite(TH), TH, 0.0)
     return Result(table=W, tol=T, pred=pred, tol_pred=tol_pred, g=gs, loss_sum=loss_sum, labelled=labelled,
-                  w0_delta=w0_delta, bad_id=bad_id)
+                  w0_delta=w0_delta, bad_id=bad_id, acc=Hm if ada else None, tol_acc=TH if ada else None)
 
 
 def objective(table, cols, fields, vals, y, *, num_features, num_fields, k, loss, reg_linear=0.0, reg_factors=0.0,

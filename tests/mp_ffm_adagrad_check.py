@@ -30,7 +30,7 @@ def _full_acc(m, dev):
 
 def check(rank, world, dev, bias):
     from fps_b200.models.fm import DeviceFieldAwareFM
-    from tests import ffm_adagrad_ref
+    from tests import ffm_ref
 
     m = DeviceFieldAwareFM(NF, F, K, learning_rate=0.05, reg_factors=0.01, init_range=(-0.3, 0.3), bias=bias, seed=3,
                            optimizer="adagrad")
@@ -52,12 +52,12 @@ def check(rank, world, dev, bias):
         for s in range(STEPS):
             for r in range(world):
                 rp, cols, fields, vals, labels = batches[r][s]
-                res = ffm_adagrad_ref.replay(W, rp, cols, fields, vals, labels, num_features=NF, num_fields=F, k=K,
-                                             lr=0.05, reg_factors=0.01, bias=False, tol=T, acc=H, acc_tol=TH)
+                res = ffm_ref.replay(W, rp, cols, fields, vals, labels, num_features=NF, num_fields=F, k=K,
+                                     lr=0.05, reg_factors=0.01, bias=False, tol=T, acc=H, acc_tol=TH)
                 W, T, H, TH = res.table, res.tol, res.acc, res.tol_acc
         for name, a, b, tol in (("table", got, W, T), ("acc", got_h, H, TH)):
             err = np.abs(a - b)
-            assert (err <= ffm_adagrad_ref.MARGIN * tol).all(), (name, (err / np.maximum(tol, 1e-30)).max())
+            assert (err <= ffm_ref.MARGIN * tol).all(), (name, (err / np.maximum(tol, 1e-30)).max())
         assert got[NF, 0] == 0.0 and (got_h[NF] == 0).all()
     else:
         parts = [None] * world

@@ -29,7 +29,7 @@ def _full_acc(m, dev):
 
 def check(rank, world, dev, bias):
     from fps_b200.models.fm import DeviceFactorizationMachine
-    from tests import fm_adagrad_ref
+    from tests import fm_ref
 
     m = DeviceFactorizationMachine(NF, K, learning_rate=0.05, reg_factors=0.01, init_range=(-0.3, 0.3), bias=bias,
                                    seed=3, optimizer="adagrad")
@@ -53,14 +53,13 @@ def check(rank, world, dev, bias):
         for s in range(STEPS):
             for r in range(world):
                 rp, cols, vals, labels = batches[r][s]
-                res = fm_adagrad_ref.replay(W, rp, cols, vals, labels, num_features=NF, dim=1 + K, lr=0.05,
-                                            reg_factors=0.01, bias=False, tol=T, acc=H, acc_tol=TH)
+                res = fm_ref.replay(W, rp, cols, vals, labels, num_features=NF, dim=1 + K, lr=0.05,
+                                    reg_factors=0.01, bias=False, tol=T, acc=H, acc_tol=TH)
                 W, T, H, TH = res.table, res.tol, res.acc, res.tol_acc
         d = 1 + K
         for name, a, b, tol in (("table", got, W, T), ("acc", got_h, H, TH)):
             err = np.abs(a - b[:, :d])
-            assert (err <= fm_adagrad_ref.MARGIN * tol[:, :d]).all(), (name,
-                                                                       (err / np.maximum(tol[:, :d], 1e-30)).max())
+            assert (err <= fm_ref.MARGIN * tol[:, :d]).all(), (name, (err / np.maximum(tol[:, :d], 1e-30)).max())
         assert got[NF, 0] == 0.0 and (got_h[NF] == 0).all()
     else:
         parts = [None] * world

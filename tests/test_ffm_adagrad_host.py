@@ -1,4 +1,4 @@
-"""AdaGrad in the field-aware FM's fp64 replay (tests/ffm_adagrad_ref.py, DESIGN §2.17) against autograd, its breaks, a
+"""AdaGrad in the field-aware FM's fp64 replay (tests/ffm_ref.py, DESIGN §2.17) against autograd, its breaks, a
 planted field-aware model at libffm's settings, the refusals of the binding and model, and the ``acc`` field of
 ``FfmArgs``.  No GPU."""
 import ctypes as C
@@ -10,7 +10,7 @@ import torch
 import fps_b200  # noqa: F401
 from fps_b200.models.fm import DeviceFieldAwareFM, check_ffm_config, roc_auc
 from fps_b200.ops import native
-from tests import ffm_adagrad_ref, ffm_ref, fm_adagrad_ref
+from tests import ffm_ref, fm_ref
 from tests.test_ffm_host import (NF, QUALITY, QUALITY_SEED, _args, _example, initial_ffm_table,  # noqa: F401
                                  no_library, planted)
 from tests.test_native_records_host import _layout, _nvcc
@@ -51,7 +51,7 @@ def test_update_is_adagrad_of_the_gradient(loss, k, F, reg):
     y = 1.0 if loss == "logistic" else 0.7
     lr = 0.5
     kw = dict(num_features=NF, num_fields=F, k=k, loss=loss, reg_linear=reg[0], reg_factors=reg[1])
-    r = ffm_adagrad_ref.replay(W, [0, len(cols)], cols, fields, vals, [y], lr=lr, fp32=False, acc=H, **kw)
+    r = ffm_ref.replay(W, [0, len(cols)], cols, fields, vals, [y], lr=lr, fp32=False, acc=H, **kw)
     t = torch.tensor(W, dtype=torch.float64, requires_grad=True)
     ffm_ref.objective(t, cols, fields, torch.from_numpy(vals), y, xp=torch, **kw).backward()
     gam = t.grad.numpy()
@@ -75,10 +75,8 @@ def test_without_acc_the_replay_is_unchanged():
     F = (W.shape[1] - 4) // ffm_ref.kpad(5)
     kw = dict(num_features=NF, num_fields=F, k=5, loss="logistic", lr=0.3, reg_linear=0.05, reg_factors=0.05)
     for extra in (dict(), dict(repull=True), dict(stale=True)):
-        a = ffm_ref.replay(W, [0, 3, len(cols)], cols, fields, vals, [1.0, 0.0], **kw, **extra)
-        b = ffm_adagrad_ref.replay(W, [0, 3, len(cols)], cols, fields, vals, [1.0, 0.0], acc=None, **kw, **extra)
-        assert all(np.array_equal(a[f], b[f]) for f in ("table", "tol", "pred", "tol_pred"))
-        assert b.acc is None
+        b = ffm_ref.replay(W, [0, 3, len(cols)], cols, fields, vals, [1.0, 0.0], acc=None, **kw, **extra)
+        assert b.acc is None and b.tol_acc is None
 
 
 def test_adagrad_breaks_change_the_replay():
@@ -87,9 +85,9 @@ def test_adagrad_breaks_change_the_replay():
     F = (W.shape[1] - 4) // ffm_ref.kpad(5)
     H = _acc_like(W, rng, F, 5)
     kw = dict(num_features=NF, num_fields=F, k=5, loss="logistic", lr=0.3, reg_linear=0.05, reg_factors=0.05, acc=H)
-    base = ffm_adagrad_ref.replay(W, [0, 2, len(cols)], cols, fields, vals, [1.0, 0.0], **kw)
-    for b in fm_adagrad_ref.ADAGRAD_BREAKS:
-        other = ffm_adagrad_ref.replay(W, [0, 2, len(cols)], cols, fields, vals, [1.0, 0.0], breaks=b, **kw)
+    base = ffm_ref.replay(W, [0, 2, len(cols)], cols, fields, vals, [1.0, 0.0], **kw)
+    for b in fm_ref.ADAGRAD_BREAKS:
+        other = ffm_ref.replay(W, [0, 2, len(cols)], cols, fields, vals, [1.0, 0.0], breaks=b, **kw)
         moved = (np.abs(other.table - base.table) > 10 * (base.tol + other.tol)).any()
         moved |= (np.abs(other.acc - base.acc) > 10 * (base.tol_acc + other.tol_acc)).any()
         assert moved, b
@@ -103,8 +101,8 @@ def test_repull_reads_h_as_the_earlier_pushes_left_it():
     W[:NF, 4:] = rng.normal(0, 0.5, (NF, F * k))
     cols, fields = np.array([1, 2, 3]), np.array([0, 1, 1])      # V[1, 1] pairs with both 2 and 3
     kw = dict(num_features=NF, num_fields=F, k=k, lr=0.5, acc=np.zeros_like(W))
-    a = ffm_adagrad_ref.replay(W, [0, 3], cols, fields, None, [1.0], **kw)
-    b = ffm_adagrad_ref.replay(W, [0, 3], cols, fields, None, [1.0], repull=True, **kw)
+    a = ffm_ref.replay(W, [0, 3], cols, fields, None, [1.0], **kw)
+    b = ffm_ref.replay(W, [0, 3], cols, fields, None, [1.0], repull=True, **kw)
     assert not np.array_equal(a.table[1], b.table[1])
 
 
@@ -131,7 +129,7 @@ def fit_replay_ffm(lr, optimizer, reg_factors=0.0, k=4):
         for b0 in range(0, n, B):
             b1 = min(b0 + B, n)
             s = slice(rp[b0], rp[b1])
-            r = ffm_adagrad_ref.replay(W, rp[b0:b1 + 1] - rp[b0], c[s], f[s], None, l[b0:b1], lr=lr, acc=H, **kw)
+            r = ffm_ref.replay(W, rp[b0:b1 + 1] - rp[b0], c[s], f[s], None, l[b0:b1], lr=lr, acc=H, **kw)
             W, H = r.table, r.acc
     pred = ffm_ref.replay(W, rp[n:] - rp[n], c[rp[n]:], f[rp[n]:], None, None, predict_only=True, **kw).pred
     return roc_auc(pred, l[n:])

@@ -1,4 +1,4 @@
-"""AdaGrad in the factorization machine's fp64 replay (tests/fm_adagrad_ref.py, DESIGN §2.17) against autograd, its breaks
+"""AdaGrad in the factorization machine's fp64 replay (tests/fm_ref.py, DESIGN §2.17) against autograd, its breaks
 and error model, a planted model, the refusals of the binding and model, and the ``acc`` field of ``FmArgs``.
 No GPU."""
 import ctypes as C
@@ -10,7 +10,7 @@ import torch
 import fps_b200  # noqa: F401
 from fps_b200.models.fm import DeviceFactorizationMachine, check_fm_config, roc_auc
 from fps_b200.ops import native
-from tests import fm_adagrad_ref, fm_ref
+from tests import fm_ref
 from tests.philox_ref import init_rows_ref
 from tests.test_fm_host import NF, QUALITY, QUALITY_SEED, _args, _example, no_library, planted  # noqa: F401
 from tests.test_native_records_host import _layout, _nvcc
@@ -35,7 +35,7 @@ def test_update_is_adagrad_of_the_gradient(loss, k, reg):
     y = 1.0 if loss == "logistic" else 0.7
     lr = 0.5
     kw = dict(num_features=NF, dim=1 + k, loss=loss, reg_linear=reg[0], reg_factors=reg[1])
-    r = fm_adagrad_ref.replay(W, [0, len(cols)], cols, vals, [y], lr=lr, fp32=False, acc=H, **kw)
+    r = fm_ref.replay(W, [0, len(cols)], cols, vals, [y], lr=lr, fp32=False, acc=H, **kw)
     t = torch.tensor(W[:, : 1 + k], dtype=torch.float64, requires_grad=True)
     fm_ref.objective(t, torch.from_numpy(cols), torch.from_numpy(vals), y, xp=torch, **kw).backward()
     gam = t.grad.numpy()
@@ -54,12 +54,10 @@ def test_without_acc_the_replay_is_unchanged():
     rng = np.random.default_rng(2)
     W, cols, vals = _example(6, True, rng)
     kw = dict(num_features=NF, dim=7, loss="logistic", lr=0.3, reg_linear=0.05, reg_factors=0.05)
-    a = fm_ref.replay(W, [0, 3, 6], cols, vals, [1.0, 0.0], **kw)
-    b = fm_adagrad_ref.replay(W, [0, 3, 6], cols, vals, [1.0, 0.0], acc=None, acc_tol=None, **kw)
-    assert all(np.array_equal(a[f], b[f]) for f in ("table", "tol", "pred", "tol_pred"))
+    b = fm_ref.replay(W, [0, 3, 6], cols, vals, [1.0, 0.0], acc=None, acc_tol=None, **kw)
     assert b.acc is None and b.tol_acc is None
     with pytest.raises(ValueError, match="unknown break"):
-        fm_adagrad_ref.replay(W, [0, 3, 6], cols, vals, [1.0, 0.0], breaks="acc_abs", **kw)
+        fm_ref.replay(W, [0, 3, 6], cols, vals, [1.0, 0.0], breaks="acc_abs", **kw)
 
 
 def test_adagrad_breaks_change_the_replay():
@@ -67,9 +65,9 @@ def test_adagrad_breaks_change_the_replay():
     W, cols, vals = _example(6, False, rng)
     H = _acc_like(W, rng)
     kw = dict(num_features=NF, dim=7, loss="logistic", lr=0.3, reg_linear=0.05, reg_factors=0.05, acc=H)
-    base = fm_adagrad_ref.replay(W, [0, 2, 4], cols[:4], vals[:4], [1.0, 0.0], **kw)
-    for b in fm_adagrad_ref.ADAGRAD_BREAKS:
-        other = fm_adagrad_ref.replay(W, [0, 2, 4], cols[:4], vals[:4], [1.0, 0.0], breaks=b, **kw)
+    base = fm_ref.replay(W, [0, 2, 4], cols[:4], vals[:4], [1.0, 0.0], **kw)
+    for b in fm_ref.ADAGRAD_BREAKS:
+        other = fm_ref.replay(W, [0, 2, 4], cols[:4], vals[:4], [1.0, 0.0], breaks=b, **kw)
         moved = (np.abs(other.table - base.table) > 10 * (base.tol + other.tol)).any()
         moved |= (np.abs(other.acc - base.acc) > 10 * (base.tol_acc + other.tol_acc)).any()
         assert moved, b
@@ -84,7 +82,7 @@ def test_fp32_bound_covers_an_fp32_evaluation():
     tgam = 4 * EPS * np.abs(gam)
     gam32 = np.float32(gam * (1 + rng.choice([-1, 1], n) * 3 * EPS))   # within tgam with its own rounding
     lr = np.float32(0.2)
-    d, td, dh, tdh = fm_adagrad_ref.adagrad(gam, tgam, H, np.zeros(n), float(lr))
+    d, td, dh, tdh = fm_ref.adagrad(gam, tgam, H, np.zeros(n), float(lr))
     gg32 = gam32 * gam32
     d32 = -lr * gam32 / np.sqrt(np.float32(np.float32(1) + np.float32(H)) + gg32)
     assert d32.dtype == np.float32
@@ -113,7 +111,7 @@ def fit_replay(k, lr, optimizer, reg=(0.0, 0.0), planted_data=None):
     for _ in range(q["epochs"]):
         for b0 in range(0, n, B):
             b1 = min(b0 + B, n)
-            r = fm_adagrad_ref.replay(W, rp[b0:b1 + 1] - rp[b0], c[rp[b0]:rp[b1]], None, l[b0:b1], lr=lr, acc=H, **kw)
+            r = fm_ref.replay(W, rp[b0:b1 + 1] - rp[b0], c[rp[b0]:rp[b1]], None, l[b0:b1], lr=lr, acc=H, **kw)
             W, H = r.table, r.acc
     pred = fm_ref.replay(W, rp[n:] - rp[n], c[rp[n]:], None, None, predict_only=True, **kw).pred
     return roc_auc(pred, l[n:])

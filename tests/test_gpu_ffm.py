@@ -91,7 +91,7 @@ def _launch(m, batch, id64=False, max_ctas=0, predict_only=False):
                     num_features=m.num_features, num_fields=m.num_fields, num_factors=m.k, loss=m.loss, lr=m.lr,
                     reg_linear=m.reg_linear, reg_factors=m.reg_factors, bias=m.bias, bias_state=m._bias_state,
                     predict_only=predict_only, stats=m._stats, nan_flag=m._flags[0:1], bad_id=m._flags[1:2],
-                    max_ctas=max_ctas)
+                    max_ctas=max_ctas, acc=m._acc_c)
     torch.cuda.synchronize()
     return pred.cpu().numpy().astype(np.float64), m._flags.cpu().numpy(), m._stats.cpu().numpy()
 

@@ -1,5 +1,5 @@
-"""Field-aware FM AdaGrad kernel (``fps_ffm_adagrad_kernel``, DESIGN §2.17) against the fp64 replay of
-tests/ffm_adagrad_ref.py, launch by launch, and the public DeviceFieldAwareFM with ``optimizer="adagrad"``.
+"""Field-aware FM kernel under AdaGrad (``fps_ffm_kernel`` with ``ADA`` set, DESIGN §2.17) against the fp64 replay
+of tests/ffm_ref.py with ``acc``, launch by launch, and the public DeviceFieldAwareFM with ``optimizer="adagrad"``.
 
 Every replay case compares the table and the accumulators after one launch with the replay fed the pre-launch
 state: every element within ``MARGIN`` times its bound, the padding of both exactly zero.  Unless a case says
@@ -8,11 +8,11 @@ import numpy as np
 import pytest
 import torch
 
-from tests import ffm_adagrad_ref, ffm_ref, fm_adagrad_ref
+from tests import ffm_ref, fm_ref
 from tests.test_ffm_adagrad_host import (AUC_ADAGRAD, AUC_LIBFFM_FFM, AUC_LIBFFM_FM, AUC_LIBFFM_LINEAR, LIBFFM,
                                          QUALITY_LRS)
 from tests.test_ffm_host import QUALITY, QUALITY_SEED, planted
-from tests.test_gpu_ffm import FS, KS, _batch, _config, _nf, _padding_ok
+from tests.test_gpu_ffm import FS, KS, _batch, _config, _launch, _nf, _padding_ok
 
 pytestmark = pytest.mark.gpu
 
@@ -46,31 +46,11 @@ def _state(m):
     return (m.table.local.cpu().numpy().astype(np.float64), m._acc.local.cpu().numpy().astype(np.float64))
 
 
-def _launch(m, batch, id64=False, max_ctas=0, predict_only=False):
-    from fps_b200.ops import native
-
-    rp, cols, fields, vals, labels = batch
-    dev = m.dev
-    pred = torch.full((len(rp) - 1,), float("nan"), dtype=torch.float32, device=dev)
-    m._flags.zero_()
-    m._stats.zero_()
-    t = lambda a: torch.from_numpy(a).to(dev)
-    native.ffm_step(m.table.table_c, t(rp), t(cols.astype(np.int64 if id64 else np.int32)), t(fields),
-                    None if vals is None else t(vals), None if predict_only else t(labels), pred,
-                    num_features=m.num_features, num_fields=m.num_fields, num_factors=m.k, loss=m.loss, lr=m.lr,
-                    reg_linear=m.reg_linear, reg_factors=m.reg_factors, bias=m.bias, bias_state=m._bias_state,
-                    predict_only=predict_only, stats=m._stats, nan_flag=m._flags[0:1], bad_id=m._flags[1:2],
-                    max_ctas=max_ctas, acc=m._acc_c)
-    torch.cuda.synchronize()
-    return pred.cpu().numpy().astype(np.float64), m._flags.cpu().numpy(), m._stats.cpu().numpy()
-
-
 def _replay(m, W, H, batch, breaks=None, predict_only=False, **kw):
     rp, cols, fields, vals, labels = batch
-    return ffm_adagrad_ref.replay(W, rp, cols, fields, vals, labels, num_features=m.num_features,
-                                  num_fields=m.num_fields, k=m.k, loss=m.loss, lr=m.lr, reg_linear=m.reg_linear,
-                                  reg_factors=m.reg_factors, bias=m.bias, breaks=breaks, predict_only=predict_only,
-                                  acc=H, **kw)
+    return ffm_ref.replay(W, rp, cols, fields, vals, labels, num_features=m.num_features, num_fields=m.num_fields,
+                          k=m.k, loss=m.loss, lr=m.lr, reg_linear=m.reg_linear, reg_factors=m.reg_factors, bias=m.bias,
+                          breaks=breaks, predict_only=predict_only, acc=H, **kw)
 
 
 def _violations(r, W2, H2, pred):
@@ -230,7 +210,7 @@ def test_no_host_sync_and_one_launch_per_step():
 
 
 def test_broken_replays_fail():
-    counts = {b: 0 for b in fm_adagrad_ref.ADAGRAD_BREAKS}
+    counts = {b: 0 for b in fm_ref.ADAGRAD_BREAKS}
     cases = 0
     for i, (k, F) in enumerate([(k, F) for k in (1, 4, 5, 8, 9, 16, 17, 33, 64) for F in (2, 39)]):
         m = _model(k, F, reg=(0.05, 0.05))
@@ -240,7 +220,7 @@ def test_broken_replays_fail():
         pred, _, _ = _launch(m, batch)
         W2, H2 = _state(m)
         assert _violations(_replay(m, W, H, batch), W2, H2, pred) == 0
-        for b in fm_adagrad_ref.ADAGRAD_BREAKS:
+        for b in fm_ref.ADAGRAD_BREAKS:
             counts[b] += _violations(_replay(m, W, H, batch, breaks=b), W2, H2, pred) > 0
         cases += 1
         m.close()

@@ -1,5 +1,6 @@
-"""Factorization-machine AdaGrad kernel (``fps_fm_adagrad_kernel``, DESIGN §2.17) against the fp64 replay of
-tests/fm_adagrad_ref.py, launch by launch, and the public DeviceFactorizationMachine with ``optimizer="adagrad"``.
+"""Factorization-machine kernel under AdaGrad (``fps_fm_kernel`` with ``ADA`` set, DESIGN §2.17) against the fp64
+replay of tests/fm_ref.py with ``acc``, launch by launch, and the public DeviceFactorizationMachine with
+``optimizer="adagrad"``.
 
 Every replay case reads the table and the accumulators, runs one launch, and compares both with the replay fed the
 pre-launch state: every element within ``MARGIN`` times its bound, the padding of both exactly zero.  Unless a case
@@ -8,10 +9,10 @@ import numpy as np
 import pytest
 import torch
 
-from tests import fm_adagrad_ref, fm_ref
+from tests import fm_ref
 from tests.test_fm_adagrad_host import AUC_ADAGRAD, QUALITY_LRS
 from tests.test_fm_host import QUALITY, QUALITY_SEED, planted
-from tests.test_gpu_fm import KS, NF, _batch, _config
+from tests.test_gpu_fm import KS, NF, _batch, _config, _launch
 
 pytestmark = pytest.mark.gpu
 
@@ -42,32 +43,11 @@ def _state(m):
     return (m.table.local.cpu().numpy().astype(np.float64), m._acc.local.cpu().numpy().astype(np.float64))
 
 
-def _launch(m, batch, id64=False, max_ctas=0, predict_only=False):
-    from fps_b200.ops import native
-
-    rp, cols, vals, labels = batch
-    dev = m.dev
-    n = len(rp) - 1
-    pred = torch.full((n,), float("nan"), dtype=torch.float32, device=dev)
-    m._flags.zero_()
-    m._stats.zero_()
-    native.fm_step(m.table.table_c, torch.from_numpy(rp).to(dev),
-                   torch.from_numpy(cols.astype(np.int64 if id64 else np.int32)).to(dev),
-                   None if vals is None else torch.from_numpy(vals).to(dev),
-                   None if predict_only else torch.from_numpy(labels).to(dev), pred,
-                   num_features=m.num_features, loss=m.loss, lr=m.lr, reg_linear=m.reg_linear,
-                   reg_factors=m.reg_factors, bias=m.bias, bias_state=m._bias_state, predict_only=predict_only,
-                   stats=m._stats, nan_flag=m._flags[0:1], bad_id=m._flags[1:2], max_ctas=max_ctas,
-                   acc=m._acc_c)
-    torch.cuda.synchronize()
-    return pred.cpu().numpy().astype(np.float64), m._flags.cpu().numpy(), m._stats.cpu().numpy()
-
-
 def _replay(m, W, H, batch, breaks=None, predict_only=False, **kw):
     rp, cols, vals, labels = batch
-    return fm_adagrad_ref.replay(W, rp, cols, vals, labels, num_features=m.num_features, dim=1 + m.k, loss=m.loss,
-                                 lr=m.lr, reg_linear=m.reg_linear, reg_factors=m.reg_factors, bias=m.bias,
-                                 breaks=breaks, predict_only=predict_only, acc=H, **kw)
+    return fm_ref.replay(W, rp, cols, vals, labels, num_features=m.num_features, dim=1 + m.k, loss=m.loss,
+                         lr=m.lr, reg_linear=m.reg_linear, reg_factors=m.reg_factors, bias=m.bias, breaks=breaks,
+                         predict_only=predict_only, acc=H, **kw)
 
 
 def _violations(r, W2, H2, pred):
@@ -228,7 +208,7 @@ def test_no_host_sync_and_one_launch_per_step():
 
 
 def test_broken_replays_fail():
-    counts = {b: 0 for b in fm_adagrad_ref.ADAGRAD_BREAKS}
+    counts = {b: 0 for b in fm_ref.ADAGRAD_BREAKS}
     cases = 0
     for i, k in enumerate(KS):
         for loss in ("logistic", "squared"):
@@ -239,7 +219,7 @@ def test_broken_replays_fail():
             pred, _, _ = _launch(m, batch)
             W2, H2 = _state(m)
             assert _violations(_replay(m, W, H, batch), W2, H2, pred) == 0
-            for b in fm_adagrad_ref.ADAGRAD_BREAKS:
+            for b in fm_ref.ADAGRAD_BREAKS:
                 counts[b] += _violations(_replay(m, W, H, batch, breaks=b), W2, H2, pred) > 0
             cases += 1
             m.close()
