@@ -187,6 +187,8 @@ extern "C" int fps_ctr_step(const CtrArgs* a, float* W1, float* W1T, float* b1, 
   if (a->batch <= 0) return 0;
   const int IN = a->fields * a->emb;
   if (IN > CTR_MAX_IN || IN > CTR_H) return -1501;
+  // the wide weight is column `emb` of every pulled row: a narrower stride would read the next row's first float
+  if (a->stride < a->emb + 1) return -1801;
   const size_t smem = (size_t)(CTR_TB * IN + CTR_TB * CTR_H + 8 * CTR_TB + CTR_TB) * sizeof(float);
   cudaError_t e = cudaFuncSetAttribute(fps_ctr_tower_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return (int)e;

@@ -83,6 +83,7 @@ extern "C" const char* fps_error_string(int code) {
   if (code == -1704) return "field-aware FM: n or nnz out of range";
   if (code == -1705) return "field-aware FM: bias on without its accumulator";
   if (code == -1706) return "field-aware FM: AdaGrad accumulator table's geometry differs from the table's";
+  if (code == -1801) return "wide-&-deep tower: row stride narrower than emb + 1 (the wide weight column)";
   if (code < 0) return "fps: invalid argument";
   return cudaGetErrorString((cudaError_t)code);
 }

@@ -159,6 +159,15 @@ def _req(t: torch.Tensor, name: str, dtype=None) -> None:
         raise TypeError(f"{name} must be {dtype}, got {t.dtype}")
 
 
+def _req_vec4(t: torch.Tensor, name: str) -> None:
+    """A ``[n, w]`` row buffer with ``w % 4 == 0`` is moved in 16-byte vectors by the row kernels, so its first
+    element must sit on a 16-byte boundary.  A contiguous view with a storage offset that is not a multiple of 4
+    floats would pass ``_req`` and reach the device as misaligned vector accesses."""
+    if t.dim() == 2 and t.shape[1] % 4 == 0 and t.data_ptr() % 16 != 0:
+        raise ValueError(f"{name}: rows {t.shape[1]} floats wide must start on a 16-byte boundary "
+                         f"(storage offset {t.storage_offset()} floats); pass a copy or an aligned view")
+
+
 def _bump(n: int = 1) -> None:
     global _launch_count
     _launch_count += n
@@ -1012,9 +1021,11 @@ def pull_gather(tab: ShardTableC, ids: torch.Tensor, out: torch.Tensor, touch: b
     """``out[i] = table[ids[i]]`` (one-sided gather, K1).  Pull limiter: ``credits`` (int32 ``[2]``
     device tensor, ``credits[0]`` = pullLimit) is the device-side credit counter -- a lane-group takes a
     credit before it touches the owner and returns it when the answer is stored; ``credits[1]`` counts
-    stalls.  Without it ``max_inflight_rows`` caps the grid (static limiter)."""
+    stalls.  Without it ``max_inflight_rows`` caps the grid (static limiter).  An ``out`` whose width is a
+    multiple of 4 is stored in 16-byte vectors and must start on a 16-byte boundary (``ValueError`` otherwise)."""
     _req(ids, "ids"); _req(out, "out", torch.float32)
     assert out.shape[0] == ids.numel() and out.shape[1] <= tab.stride
+    _req_vec4(out, "out")
     if credits is not None:
         _req(credits, "credits", torch.int32)
     _check(lib().fps_pull_gather(C.byref(tab), C.c_void_p(ids.data_ptr()), _id_bytes(ids),
@@ -1028,8 +1039,11 @@ def pull_gather(tab: ShardTableC, ids: torch.Tensor, out: torch.Tensor, touch: b
 
 def push_add(tab: ShardTableC, ids: torch.Tensor, delta: torch.Tensor, scale: float = 1.0,
              touch: bool = False, nan_flag: Optional[torch.Tensor] = None) -> None:
+    """``table[ids[i]] += scale * delta[i]`` (K2).  A ``delta`` whose width is a multiple of 4 is read in 16-byte
+    vectors and must start on a 16-byte boundary (``ValueError`` otherwise)."""
     _req(ids, "ids"); _req(delta, "delta", torch.float32)
     assert delta.shape[0] == ids.numel() and delta.shape[1] <= tab.stride
+    _req_vec4(delta, "delta")
     _check(lib().fps_push_add(C.byref(tab), C.c_void_p(ids.data_ptr()), _id_bytes(ids),
                               C.c_longlong(ids.numel()), C.c_void_p(delta.data_ptr()),
                               int(delta.shape[1]), C.c_float(scale), int(bool(touch)),
@@ -1091,17 +1105,43 @@ def ctr_step(rows: torch.Tensor, labels: torch.Tensor, fields: int, emb: int, we
              prob: Optional[torch.Tensor] = None) -> None:
     """Fused wide-&-deep tower: forward, BCE, backward, dense SGD (mean gradient) and the row gradients
     (``-lr * dLoss/drow``, ready to push) in one kernel + a small apply kernel.  ``weights``: W1 [IN, 256],
-    W1T [256, IN], b1 [256], w2 [256], b2 [1]; ``grads``: same shapes minus W1T.  csrc/fps_ctr.cu."""
+    W1T [256, IN], b1 [256], w2 [256], b2 [1]; ``grads``: same shapes minus W1T.  ``rows`` is ``[B * fields,
+    stride]`` with ``stride >= emb + 1`` (column ``emb`` is the wide weight); ``d_rows`` (train) has the shape of
+    ``rows``, ``prob`` (optional) ``B`` elements, ``loss`` two.  Any other shape is a ``ValueError`` before
+    anything is launched.  csrc/fps_ctr.cu."""
     _req(rows, "rows", torch.float32); _req(labels, "labels", torch.float32); _req(loss, "loss", torch.float32)
-    a = CtrArgsC()
-    a.rows = rows.data_ptr(); a.labels = labels.data_ptr(); a.batch = labels.numel()
-    a.fields, a.emb, a.stride = int(fields), int(emb), int(rows.shape[1])
-    assert rows.shape[0] == labels.numel() * fields
-    for k in ("W1", "W1T", "b1", "w2", "b2"):
+    fields, emb = int(fields), int(emb)
+    B, IN = labels.numel(), fields * emb
+    if fields < 1 or emb < 1 or IN > CTR_HIDDEN:
+        raise ValueError(f"fields ({fields}) and emb ({emb}) must be >= 1 with fields * emb <= {CTR_HIDDEN}")
+    if rows.dim() != 2 or rows.shape[0] != B * fields or rows.shape[1] < emb + 1:
+        raise ValueError(f"rows must be [B * fields, >= emb + 1] = [{B * fields}, >= {emb + 1}], "
+                         f"got {list(rows.shape)}")
+    if loss.numel() != 2:
+        raise ValueError(f"loss must hold 2 floats, got {loss.numel()}")
+    shapes = {"W1": (IN, CTR_HIDDEN), "W1T": (CTR_HIDDEN, IN), "b1": (CTR_HIDDEN,), "w2": (CTR_HIDDEN,), "b2": (1,)}
+    for k, shp in shapes.items():
         _req(weights[k], k, torch.float32)
-        setattr(a, k, weights[k].data_ptr())
+        if tuple(weights[k].shape) != shp:
+            raise ValueError(f"weights[{k!r}] must be {list(shp)}, got {list(weights[k].shape)}")
+    if prob is not None:
+        _req(prob, "prob", torch.float32)
+        if prob.numel() != B:
+            raise ValueError(f"prob must hold B = {B} floats, got {prob.numel()}")
     if train:
         _req(d_rows, "d_rows", torch.float32)
+        if d_rows.shape != rows.shape:
+            raise ValueError(f"d_rows must have the shape of rows {list(rows.shape)}, got {list(d_rows.shape)}")
+        for k in ("W1", "b1", "w2", "b2"):
+            _req(grads[k], f"grads[{k!r}]", torch.float32)
+            if tuple(grads[k].shape) != shapes[k]:
+                raise ValueError(f"grads[{k!r}] must be {list(shapes[k])}, got {list(grads[k].shape)}")
+    a = CtrArgsC()
+    a.rows = rows.data_ptr(); a.labels = labels.data_ptr(); a.batch = B
+    a.fields, a.emb, a.stride = fields, emb, int(rows.shape[1])
+    for k in shapes:
+        setattr(a, k, weights[k].data_ptr())
+    if train:
         a.gW1, a.gb1, a.gw2, a.gb2 = (grads[k].data_ptr() for k in ("W1", "b1", "w2", "b2"))
         a.d_rows = d_rows.data_ptr()
     a.loss = loss.data_ptr()
