@@ -92,7 +92,9 @@ __device__ __forceinline__ void fps_credit_acquire(int* credits, int n = 1) {
 
 // ADA = 1: row-wise AdaGrad (DESIGN §2.10).  e is taken with learning rate 1, each row's step is
 //   s = |delta|^2 / k,  row += lr * delta / (sqrt(G + s) + eps),  G += s
-// with G the row's accumulator as pulled next to the row.  ADA = 0 is the SGD step, unchanged.
+// with G the row's accumulator as pulled next to the row.  ADA = 0 is the SGD step, unchanged.  AdaGrad runs
+// only the default register-staged geometries (no L2 hints, output stream or credit counter; a pull limit is the
+// static capped grid).
 template <typename IdT, int LPR, int VPL, int R, int FMT, int HINT, int EMIT, int LIMIT, int ADA>
 __device__ __forceinline__ void fps_mf_step_body(const MfArgs& a) {
   unsigned long long pol_user = 0, pol_item = 0;
@@ -269,18 +271,13 @@ __device__ __forceinline__ void fps_mf_step_body(const MfArgs& a) {
   if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
 }
 
-template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT, int HINT = 0, int EMIT = 0, int LIMIT = 0>
+// The step is a function the kernel calls, not the kernel's own body: written out in the kernel, it compiles to
+// other register assignments in some 64-bit-id instantiations.
+template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT, int HINT = 0, int EMIT = 0, int LIMIT = 0,
+          int ADA = 0>
 __global__ void __launch_bounds__(256, MINB)
     fps_mf_sgd_fused_kernel(const __grid_constant__ MfArgs a) {
-  fps_mf_step_body<IdT, LPR, VPL, R, FMT, HINT, EMIT, LIMIT, 0>(a);
-}
-
-// Row-wise AdaGrad family: the default register-staged geometries only (no L2 hints, output stream or
-// credit counter; a pull limit is the static capped grid).
-template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT>
-__global__ void __launch_bounds__(256, MINB)
-    fps_mf_adagrad_fused_kernel(const __grid_constant__ MfArgs a) {
-  fps_mf_step_body<IdT, LPR, VPL, R, FMT, 0, 0, 0, 1>(a);
+  fps_mf_step_body<IdT, LPR, VPL, R, FMT, HINT, EMIT, LIMIT, ADA>(a);
 }
 
 // A lane-group keeps R records, and so R row pairs, in flight.
@@ -288,9 +285,7 @@ template <typename IdT, int LPR, int VPL, int R, int MINB, int FMT, int HINT = 0
           int ADA = 0>
 static int launch_mf(const MfArgs& a, int max_inflight_rows, int num_sms, cudaStream_t stream) {
   const int threads = 256;
-  void (*kern)(const MfArgs);
-  if constexpr (ADA) kern = fps_mf_adagrad_fused_kernel<IdT, LPR, VPL, R, MINB, FMT>;
-  else kern = fps_mf_sgd_fused_kernel<IdT, LPR, VPL, R, MINB, FMT, HINT, EMIT, LIMIT>;
+  auto kern = fps_mf_sgd_fused_kernel<IdT, LPR, VPL, R, MINB, FMT, HINT, EMIT, LIMIT, ADA>;
   const long long blocks = fps_row_grid(kern, threads, threads / LPR, num_sms, a.reserve_total, max_inflight_rows, R,
                                         a.n_pos * (1 + a.neg_rate), R);
   kern<<<(int)blocks, threads, 0, stream>>>(a);

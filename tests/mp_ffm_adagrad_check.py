@@ -39,6 +39,7 @@ def check(rank, world, dev, bias):
     W, H = _full_table(m, dev), _full_acc(m, dev)
     batches = _batches(rank, world)
     t = lambda a: torch.from_numpy(a).to(dev)
+    dist.barrier()   # every rank has read the starting table before any rank pushes to it
     for s in range(STEPS):
         rp, cols, fields, vals, labels = batches[rank][s]
         m.step_csr(t(rp), t(cols), t(fields), t(vals), t(labels))

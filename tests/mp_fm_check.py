@@ -54,6 +54,7 @@ def check(rank, world, dev, bias):
     W = np.pad(W, ((0, 0), (0, stride - W.shape[1])))
     batches = _batches(rank, world)
     t = lambda a: torch.from_numpy(a).to(dev)
+    dist.barrier()   # every rank has read the starting table before any rank pushes to it
     for s in range(STEPS):
         rp, cols, vals, labels = batches[rank][s]
         m.step_csr(t(rp), t(cols), t(vals), t(labels))

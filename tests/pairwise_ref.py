@@ -1,7 +1,6 @@
-"""fp64 replays of the pairwise MF steps (``fps_mf_bpr_kernel``, ``fps_mf_bpr_adagrad_kernel``,
-``fps_mf_warp_kernel``) and of the pointwise row-wise AdaGrad step (``fps_mf_adagrad_fused_kernel``), each with a
-first-order bound on every table element, accumulator and stat.  CPU only: the GPU suites feed them the fp32 rows the
-kernel pulls, as float64 arrays of the logical ``k`` columns.
+"""fp64 replays of the pairwise MF steps (``fps_mf_bpr_kernel`` under SGD and row-wise AdaGrad,
+``fps_mf_warp_kernel``), each with a first-order bound on every table element, accumulator and stat.  CPU only: the
+GPU suites feed them the fp32 rows the kernel pulls, as float64 arrays of the logical ``k`` columns.
 
 Where the fp32 kernels round (unit roundoff EPS = 2^-24, round to nearest; ``ops/build.py`` builds without
 fast-math, so ``sqrtf`` and ``/`` are correctly rounded):
@@ -41,9 +40,10 @@ def geometry(stride, max_nvec=128):
     return lpr, -(-nvec // lpr)
 
 
-def dot_depth(stride, max_nvec=128):
-    lpr, vpl = geometry(stride, max_nvec)
-    return 5 * vpl + int(math.log2(lpr))
+def dot_depth(stride, lpr):
+    """Depth of the kernels' fp32 dot over rows of ``stride`` floats on ``lpr`` lanes: each lane's running sum of
+    ceil(nvec / lpr) float4 dots (an FMUL, three FFMAs and an add each), then log2(lpr) shuffle adds."""
+    return 5 * -(-(stride // 4) // lpr) + int(math.log2(lpr))
 
 
 def sampled_candidates(n_pos, items, T, num_items, step, seed):
@@ -107,7 +107,7 @@ def bpr_replay(u, vi, vj, negs, lr, reg, stride, ada=None):
     ``count``, ``xpos_lo`` / ``xpos_hi`` (the ``x > 0`` count, the bound admitting either side at ``x`` near 0); and
     ``smooth`` (every AdaGrad step's relative bound below 1e-3)."""
     P, T, k = vj.shape
-    depth = dot_depth(stride)
+    depth = dot_depth(stride, geometry(stride)[0])
     lr32, reg32 = f32(lr), f32(reg)
     rate, decay = (1.0, reg32) if ada is not None else (lr32, lr32 * reg32)
     d_decay = 0.0 if ada is not None else EPS * decay          # lr * reg rounded once
@@ -223,7 +223,7 @@ def warp_replay(u, vi, vj, live, lr, reg, margin, rank_items, stride):
     ``examined``; and ``decided`` [P]: every examined ``x`` is farther from the margin than MARGIN times its bound,
     so the violator is the same in any fp32 evaluation."""
     P, T, k = vj.shape
-    depth = dot_depth(stride)
+    depth = dot_depth(stride, geometry(stride)[0])
     lr32, m32 = f32(lr), f32(margin)
     decay = lr32 * f32(reg)
     active = np.ones(P, dtype=bool)
@@ -271,58 +271,3 @@ def warp_replay(u, vi, vj, live, lr, reg, margin, rank_items, stride):
                   tol_vi=np.where(h, ti, 0.0), vs=np.where(h, vs1, vs), tol_vs=np.where(h, tj, 0.0),
                   loss=loss, tol_loss=dlt[hit].sum() + (P + 1) * EPS * loss, updated=int(hit.sum()),
                   examined=int(n.sum()))
-
-
-# ---- pointwise row-wise AdaGrad --------------------------------------------------------------------------------
-
-def _sigmoid_err(x):
-    """Relative error of the kernel's 1 / (1 + __expf(-x)): a quarter of __expf's, plus the add and the division."""
-    return 0.25 * (2.0 + 1.173 * np.abs(x)) * ULP + 2 * EPS
-
-
-def pointwise_adagrad_replay(u0, v0, r, Gu, Gv, lr, err_mode, stride, k):
-    """One ``mf_sgd_fused(item_acc=..., user_acc=...)`` launch over independent records: ``e`` at rate 1 from the
-    error rule, ``delta_u = e v``, ``delta_v = e u``, and per row ``s = |delta|^2 / k``, ``row += lr delta /
-    (sqrt(G + s) + 1e-8)``, ``G += s``.  Returns a :class:`Result` with ``u``, ``v``, ``Gu``, ``Gv`` and their
-    ``tol_*``, ``resid`` / ``tol_resid`` (the loss stat's terms), and ``e_ok``: ``|e|`` above MARGIN times its
-    bound, so the step's direction is settled where ``G`` is 0."""
-    depth = dot_depth(stride, 256)
-    d = (u0 * v0).sum(1)
-    dd = depth * EPS * np.abs(u0 * v0).sum(1)
-    resid = r - d
-    dres = dd + EPS * np.abs(resid)
-    if err_mode == 0:
-        e = _sig(resid)
-        de = 0.25 * dres + _sigmoid_err(resid)
-    elif err_mode == 1:
-        e, de = resid, dres
-    else:
-        e = r - _sig(d)
-        de = 0.25 * dd + _sigmoid_err(d) + EPS * np.abs(e)
-    nu, nv = (u0 * u0).sum(1), (v0 * v0).sum(1)
-    dnu, dnv = depth * EPS * nu, depth * EPS * nv
-    ee = e * e / k                                                # g * g / (float)dim: two roundings
-    dee = 2 * np.abs(e) * de / k + 2 * EPS * ee
-    lr32 = f32(lr)
-    res = Result(resid=resid, tol_resid=dres, e_ok=bool((np.abs(e) > MARGIN * de).all()))
-    for name, row, other, G, nrm, dnrm in (("u", u0, v0, Gu, nv, dnv), ("v", v0, u0, Gv, nu, dnu)):
-        s = ee * nrm
-        ds = dee * nrm + ee * dnrm + EPS * s
-        G = G.astype(np.float64)
-        st, dst, _ = _step(lr32, G, 0.0, s, ds)
-        gr = e * st
-        dgr = np.abs(e) * dst + st * de + EPS * np.abs(gr)
-        upd = gr[:, None] * other
-        new = row + upd
-        res[name] = new
-        res["tol_" + name] = np.abs(other) * dgr[:, None] + EPS * np.abs(upd) + EPS * np.abs(new)
-        key = "G" + name
-        res[key] = G + s
-        res["tol_" + key] = ds + EPS * (G + s)
-    return res
-
-
-def loss_bound(resid, dres):
-    """The pointwise loss stat, an fp32 sum of squared residuals in any order."""
-    sq = resid * resid
-    return (2 * np.abs(resid) * dres + dres * dres).sum() + (len(resid) + 1) * EPS * sq.sum()

@@ -1,6 +1,6 @@
-"""The pairwise MF steps (``fps_mf_bpr_kernel``, ``fps_mf_bpr_adagrad_kernel``, ``fps_mf_warp_kernel``) and the pointwise
-row-wise AdaGrad step (``fps_mf_adagrad_fused_kernel``) against the fp64 replays of ``tests/pairwise_ref.py``, at
-every dispatch rung, through the native bindings.
+"""The pairwise MF steps (``fps_mf_bpr_kernel`` under SGD and row-wise AdaGrad, ``fps_mf_warp_kernel``) and the
+pointwise row-wise AdaGrad step (``fps_mf_sgd_fused_kernel`` with ``ADA``) against the fp64 replays of
+``tests/pairwise_ref.py`` and ``tests/pointwise_ref.py``, at every dispatch rung, through the native bindings.
 
 Every case is built so that its result does not depend on the order the lane-groups run in: each row is read and
 written by one positive (a negative repeated inside one positive's list is replayed in list order), or, for hot rows,
@@ -15,9 +15,9 @@ import torch
 
 import fps_b200  # noqa: F401
 from fps_b200.ops import native
-from tests.pairwise_ref import (MARGIN, bpr_replay, geometry, pointwise_adagrad_replay, loss_bound,
-                                sampled_candidates, warp_replay)
+from tests.pairwise_ref import MARGIN, bpr_replay, geometry, sampled_candidates, warp_replay
 from tests.philox_ref import k5_negative
+from tests.pointwise_ref import loss_bound, replay as pointwise_replay
 from tests.test_gpu_mf_pointwise_edges import SEED, STEP, Guarded, _check_table, _ids, _shift_covering_steps, _table
 
 pytestmark = pytest.mark.gpu
@@ -374,8 +374,8 @@ def _pw_adagrad(dev, dim, form, err_mode, *, user_div=1, user_sharded=False, n=2
                         user_acc=native.local_table(Ua.t, 1) if user_sharded else Ua.t.view(-1), **kw)
     torch.cuda.synchronize()
     ts, ti = torch.from_numpy(slots).to(dev), torch.from_numpy(items).to(dev)
-    res = pointwise_adagrad_replay(_np(U0[ts, :dim]), _np(V0[ti, :dim]), r.astype(np.float64), _np(Ua0[ts, 0]),
-                                   _np(Va0[ti, 0]), lr, err_mode, _stride(dim), dim)
+    res = pointwise_replay(_np(U0[ts, :dim]), _np(V0[ti, :dim]), r.astype(np.float64), lr, err_mode,
+                           _rung(dim, 256)[0], acc=(_np(Ua0[ts, 0]), _np(Va0[ti, 0])))
     assert res.e_ok
     _within(_rows(U, slots, dim), res.u, res.tol_u, "user rows", "pointwise_adagrad")
     _within(_rows(V, items, dim), res.v, res.tol_v, "item rows", "pointwise_adagrad")
@@ -563,8 +563,8 @@ def test_pointwise_adagrad_sampled_negatives_match_the_replay(dev, form, neg_rat
     r = np.concatenate([np.ones(len(kp))] + [np.zeros(len(kp))] * neg_rate)
     rows = np.concatenate([items[kp]] + [negs[kp, j] for j in range(neg_rate)])
     tr = torch.from_numpy(rows).to(dev)
-    res = pointwise_adagrad_replay(u_all, np.zeros_like(u_all), r, np.zeros(len(r)), _np(Va0[tr, 0]), lr, 2,
-                                   _stride(dim), dim)
+    res = pointwise_replay(u_all, np.zeros_like(u_all), r, lr, 2, _rung(dim, 256)[0],
+                           acc=(np.zeros(len(r)), _np(Va0[tr, 0])))
     assert res.e_ok
     _within(_rows(V, rows, dim), res.v, res.tol_v, "drawn rows", "pointwise_adagrad")
     _within(_np(Va.t[tr, 0]), res.Gv, res.tol_Gv, "drawn G", "pointwise_adagrad")

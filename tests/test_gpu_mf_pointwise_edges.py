@@ -1,13 +1,11 @@
 """The pointwise MF step (``fps_mf_sgd_fused_kernel``, the TMA kernel ``fps_mf_sgd_tma_kernel`` and the fp64 kernel
-``fps_mf_sgd_fused_f64_kernel``) against an fp64 replay of the same step, at every dispatch rung, with in-kernel
-negatives replayed by ``tests/philox_ref.py``.
+``fps_mf_sgd_fused_f64_kernel``) against an fp64 replay of the same step (``tests/pointwise_ref.py``), at every
+dispatch rung, with in-kernel negatives replayed by ``tests/philox_ref.py``.
 
 Every case is built so that its result does not depend on the order the lane-groups run in: each row is read and
 written by one record (or, for hot rows, only on coordinates that one record owns), so the replay applies the records
 independently.  Every table is a slice of a larger tensor whose guard rows hold a sentinel; each case checks that the
 guard rows, the padding columns and the rows outside the batch are bitwise unchanged."""
-import math
-
 import numpy as np
 import pytest
 import torch
@@ -15,6 +13,7 @@ import torch
 import fps_b200  # noqa: F401
 from fps_b200.ops import native
 from tests.philox_ref import init_rows_f64_ref, k5_negative, philox4x32
+from tests.pointwise_ref import MARGIN, loss_bound, replay
 
 pytestmark = pytest.mark.gpu
 
@@ -52,55 +51,6 @@ def _stride(dim):
 def _tma_lpr(nvec):
     """dispatch_tma (csrc/fps_mf_tma.cu): one lane per float4 up to 32 lanes."""
     return min(32, 1 << max(0, nvec - 1).bit_length())
-
-
-# ---- tolerance ------------------------------------------------------------------------------------------------
-# The kernel computes, per record, in fp32: d = u.v as a lane's running sum of ceil(nvec / LPR) float4 dots (an FMA
-# chain of 4 and an add each: 5 roundings deep per float4) and a tree sum over the LPR lanes; resid = r - d; e from
-# resid or d; g = lr * e; u += g v and v += g u by one product and one reduction each.  A sum of depth n is within
-# n * EPS * sum|u_i v_i| of the exact dot.  __expf(x) is within (2 + 1.173 |x|) ulp (CUDA C Programming Guide,
-# intrinsic functions), a relative 2^-23 per ulp; the sigmoid 1 / (1 + E) moves by at most a quarter of E's relative
-# error, and its add and division by EPS each.  The replay carries these bounds through to every table element (first
-# order); MARGIN covers the second-order terms.
-MARGIN = 2.0
-
-
-def _sigmoid_err(x):
-    return 0.25 * (2.0 + 1.173 * np.abs(x)) * 2.0 ** -23 + 2 * EPS
-
-
-def _replay(u0, v0, r, lr, err_mode, lpr):
-    """The step of independent records: ``u0``, ``v0`` ``[n, dim]`` float64 holding the fp32 rows each record pulls,
-    ``r`` the ratings as the kernel reads them.  Returns (u1, v1, tol_u, tol_v, resid, tol_resid)."""
-    nvec = (u0.shape[1] + 3) // 4
-    depth = 5 * -(-nvec // lpr) + int(math.log2(lpr))
-    lr32 = float(np.float32(lr))
-    d = (u0 * v0).sum(1)
-    dd = depth * EPS * np.abs(u0 * v0).sum(1)
-    resid = r - d
-    dres = dd + EPS * np.abs(resid)
-    if err_mode == 0:
-        e = 1.0 / (1.0 + np.exp(-resid))
-        de = 0.25 * dres + _sigmoid_err(resid)
-    elif err_mode == 1:
-        e, de = resid, dres
-    else:
-        e = r - 1.0 / (1.0 + np.exp(-d))
-        de = 0.25 * dd + _sigmoid_err(d) + EPS * np.abs(e)
-    g = lr32 * e
-    dg = lr32 * de + EPS * np.abs(g)
-    u1 = u0 + g[:, None] * v0
-    v1 = v0 + g[:, None] * u0
-    tol_u = dg[:, None] * np.abs(v0) + 2 * EPS * (np.abs(g[:, None] * v0) + np.abs(u1))
-    tol_v = dg[:, None] * np.abs(u0) + 2 * EPS * (np.abs(g[:, None] * u0) + np.abs(v1))
-    return u1, v1, tol_u, tol_v, resid, dres
-
-
-def _loss_bound(resid, dres):
-    """stats[0] = fp32 sum of the squared residuals in any order: each square is off by 2 |resid| dres (+ its
-    rounding), and a sum of n terms in any order by n * EPS * sum."""
-    sq = resid * resid
-    return MARGIN * ((2 * np.abs(resid) * dres + dres * dres).sum() + (len(resid) + 1) * EPS * sq.sum())
 
 
 def _within(got, want, tol, what):
@@ -192,14 +142,14 @@ def _pointwise(dev, dim, form, err_mode, *, lpr, n=3000, rows=3600, seed=0, lr=0
     s, it = slots[live], items[live]
     u0 = U0[torch.from_numpy(s).to(dev), :dim].double().cpu().numpy()
     v0 = V0[torch.from_numpy(it).to(dev), :dim].double().cpu().numpy()
-    u1, v1, tu, tv, resid, dres = _replay(u0, v0, r[live].astype(np.float64), lr, err_mode, lpr)
-    _within(U.t[torch.from_numpy(s).to(dev), :dim].double().cpu().numpy(), u1, tu, "user rows")
-    _within(V.t[torch.from_numpy(it).to(dev), :dim].double().cpu().numpy(), v1, tv, "item rows")
+    res = replay(u0, v0, r[live].astype(np.float64), lr, err_mode, lpr)
+    _within(U.t[torch.from_numpy(s).to(dev), :dim].double().cpu().numpy(), res.u, res.tol_u, "user rows")
+    _within(V.t[torch.from_numpy(it).to(dev), :dim].double().cpu().numpy(), res.v, res.tol_v, "item rows")
     _check_table(U, U0, dim, s, "user table")
     _check_table(V, V0, dim, it, "item table")
     st = stats.cpu().numpy().astype(np.float64)
     assert st[1] == live.sum()
-    assert abs(st[0] - (resid * resid).sum()) <= _loss_bound(resid, dres)
+    assert abs(st[0] - (res.resid * res.resid).sum()) <= MARGIN * loss_bound(res.resid, res.tol_resid)
     assert int(nan.item()) == 0
     return U, V, users
 

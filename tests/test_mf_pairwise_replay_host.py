@@ -1,6 +1,6 @@
-"""The fp64 replays of ``tests/pairwise_ref.py`` on the CPU: equal to the project's numpy references
-(``models/mf/common.py``: ``bpr_delta``, ``warp_delta``, ``rowwise_adagrad``) on random small cases, and within their
-own reported bound of a brute-force fp32 evaluation of the same expressions."""
+"""The fp64 replays of ``tests/pairwise_ref.py`` and ``tests/pointwise_ref.py`` on the CPU: equal to the project's
+numpy references (``models/mf/common.py``: ``bpr_delta``, ``warp_delta``, ``rowwise_adagrad``) on random small cases,
+and within their own reported bound of a brute-force fp32 evaluation of the same expressions."""
 import math
 
 import numpy as np
@@ -8,9 +8,9 @@ import pytest
 
 import fps_b200  # noqa: F401
 from fps_b200.models.mf.common import bpr_delta, rowwise_adagrad, warp_delta
-from tests.pairwise_ref import (MARGIN, bpr_replay, f32, pointwise_adagrad_replay, sampled_candidates,
-                                warp_replay)
+from tests.pairwise_ref import MARGIN, bpr_replay, f32, geometry, sampled_candidates, warp_replay
 from tests.philox_ref import k5_negative
+from tests.pointwise_ref import replay as pointwise_replay
 
 F = np.float32
 
@@ -222,11 +222,12 @@ def test_warp_replay_rank_estimate_can_be_zero():
     _close(res.u, u - f32(0.1) * f32(0.01) * u, "decay only")
 
 
-# ---- pointwise AdaGrad ------------------------------------------------------------------------------------------
+# ---- pointwise, SGD and row-wise AdaGrad ------------------------------------------------------------------------
 
+@pytest.mark.parametrize("ada", [False, True])
 @pytest.mark.parametrize("err_mode", [0, 1, 2])
 @pytest.mark.parametrize("k,stride", [(3, 4), (29, 32), (509, 512), (1021, 1024)])
-def test_pointwise_adagrad_replay_matches_numpy_reference_and_fp32(err_mode, k, stride):
+def test_pointwise_replay_matches_numpy_reference_and_fp32(err_mode, k, stride, ada):
     rng = np.random.default_rng(k + err_mode)
     P = 50
     u0, v0 = _rows(rng, (P, k), k ** -0.25), _rows(rng, (P, k), k ** -0.25)
@@ -234,26 +235,34 @@ def test_pointwise_adagrad_replay_matches_numpy_reference_and_fp32(err_mode, k, 
     Gu = np.where(rng.random(P) < 0.5, rng.random(P), 0.0).astype(F).astype(np.float64)
     Gv = rng.random(P).astype(F).astype(np.float64)
     lr = f32(0.1)
-    res = pointwise_adagrad_replay(u0, v0, r, Gu, Gv, lr, err_mode, stride, k)
-    assert res.e_ok
+    res = pointwise_replay(u0, v0, r, lr, err_mode, geometry(stride, 256)[0], acc=(Gu, Gv) if ada else None)
     d = (u0 * v0).sum(1)
     e = {0: 1 / (1 + np.exp(-(r - d))), 1: r - d, 2: r - 1 / (1 + np.exp(-d))}[err_mode]
-    for p in range(P):
-        nu, su = rowwise_adagrad(u0[p], Gu[p], e[p] * v0[p], lr, k)
-        nv, sv = rowwise_adagrad(v0[p], Gv[p], e[p] * u0[p], lr, k)
-        _close(res.u[p], nu, "u")
-        _close(res.v[p], nv, "v")
-        assert math.isclose(res.Gu[p], Gu[p] + su, rel_tol=1e-12)
-        assert math.isclose(res.Gv[p], Gv[p] + sv, rel_tol=1e-12)
+    if ada:
+        assert res.e_ok
+        for p in range(P):
+            nu, su = rowwise_adagrad(u0[p], Gu[p], e[p] * v0[p], lr, k)
+            nv, sv = rowwise_adagrad(v0[p], Gv[p], e[p] * u0[p], lr, k)
+            _close(res.u[p], nu, "u")
+            _close(res.v[p], nv, "v")
+            assert math.isclose(res.Gu[p], Gu[p] + su, rel_tol=1e-12)
+            assert math.isclose(res.Gv[p], Gv[p] + sv, rel_tol=1e-12)
+    else:
+        assert res.Gu is None and res.Gv is None and res.tol_Gu is None and res.tol_Gv is None and res.e_ok is None
+        _close(res.u, u0 + (lr * e)[:, None] * v0, "u")
+        _close(res.v, v0 + (lr * e)[:, None] * u0, "v")
     # fp32
     U, V = u0.astype(F), v0.astype(F)
     d32 = (U * V).sum(1, dtype=F)
     rr = r.astype(F)
     e32 = {0: _sig32(rr - d32), 1: rr - d32, 2: rr - _sig32(d32)}[err_mode]
-    ee = e32 * e32 / F(k)
-    su, sv = ee * (V * V).sum(1, dtype=F), ee * (U * U).sum(1, dtype=F)
-    gu = e32 * (F(lr) / (np.sqrt(Gu.astype(F) + su) + F(1e-8)))
-    gv = e32 * (F(lr) / (np.sqrt(Gv.astype(F) + sv) + F(1e-8)))
+    if ada:
+        ee = e32 * e32 / F(k)
+        su, sv = ee * (V * V).sum(1, dtype=F), ee * (U * U).sum(1, dtype=F)
+        gu = e32 * (F(lr) / (np.sqrt(Gu.astype(F) + su) + F(1e-8)))
+        gv = e32 * (F(lr) / (np.sqrt(Gv.astype(F) + sv) + F(1e-8)))
+    else:
+        gu = gv = F(lr) * e32
     _within(U + gu[:, None] * V, res.u, res.tol_u, "fp32 u")
     _within(V + gv[:, None] * U, res.v, res.tol_v, "fp32 v")
 

@@ -7,7 +7,7 @@ import torch
 
 import fps_b200  # noqa: F401
 from fps_b200.ops import native
-from tests.test_gpu_mf_pointwise_edges import _replay
+from tests.pointwise_ref import replay as pointwise_replay
 from tests.window_ref import MARGIN, lanes, partition, replay, stats_bound
 
 F = np.float32
@@ -92,10 +92,10 @@ def test_chain_of_one_is_the_pointwise_replay(err_mode, k, stride):
     items = rng.permutation(n)
     lpr = lanes(stride)
     rep = replay(u0, v0, [(np.arange(n), items, r)], 0.05, err_mode, lpr)
-    u1, v1, tu, tv, resid, dres = _replay(u0, v0[items], r, 0.05, err_mode, lpr)
-    assert np.array_equal(rep["U"], u1) and np.array_equal(rep["tU"], tu)
-    assert np.array_equal(rep["V"][items], v1) and np.array_equal(rep["tV"][items], tv)
-    assert rep["sq"][0] == (resid * resid).sum() and rep["cnt"][0] == n
+    one = pointwise_replay(u0, v0[items], r, 0.05, err_mode, lpr)
+    assert np.array_equal(rep["U"], one.u) and np.array_equal(rep["tU"], one.tol_u)
+    assert np.array_equal(rep["V"][items], one.v) and np.array_equal(rep["tV"][items], one.tol_v)
+    assert rep["sq"][0] == (one.resid * one.resid).sum() and rep["cnt"][0] == n
     assert rep["groups"] == [(0, 1, False)] and rep["attempts"] == 1
 
 

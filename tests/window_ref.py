@@ -18,9 +18,9 @@ An item row's error grows with every link of its chain: the next dot sees ``sum 
 rounding.  A singleton pulls rows that other records of its micro-batch may already have pushed to: its dots carry
 those pushes' magnitudes as a further bound, and its reductions one rounding each.  Every bound is first order; the
 suite compares with ``MARGIN`` times it."""
-import math
-
 import numpy as np
+
+from tests.pointwise_ref import dot_depth, grad
 
 EPS = 2.0 ** -24          # fp32 unit roundoff
 MARGIN = 2.0
@@ -33,16 +33,6 @@ def lanes(stride):
     if not 1 <= nvec <= 32:
         raise ValueError(f"no window bucket for {nvec} float4")
     return 1 << max(0, nvec - 1).bit_length()
-
-
-def dot_depth(lpr):
-    return 5 + int(math.log2(lpr))
-
-
-def sigmoid_err(x):
-    """1 / (1 + __expf(-x)) against the exact sigmoid: a quarter of __expf's relative error, the add and the
-    division (as ``test_gpu_mf_pointwise_edges._sigmoid_err``)."""
-    return 0.25 * (2.0 + 1.173 * np.abs(x)) * 2.0 ** -23 + 2 * EPS
 
 
 def partition(batches):
@@ -74,22 +64,6 @@ def partition(batches):
     return groups, attempts
 
 
-def _grad(r, d, dd, lr32, err_mode):
-    """(resid, dres, g, dg) of fps_mf_grad from d and its bound."""
-    resid = r - d
-    dres = dd + EPS * np.abs(resid)
-    if err_mode == 0:
-        e = 1.0 / (1.0 + np.exp(-resid))
-        de = 0.25 * dres + sigmoid_err(resid)
-    elif err_mode == 1:
-        e, de = resid, dres
-    else:
-        e = r - 1.0 / (1.0 + np.exp(-d))
-        de = 0.25 * dd + sigmoid_err(d) + EPS * np.abs(e)
-    g = lr32 * e
-    return resid, dres, g, lr32 * de + EPS * np.abs(g)
-
-
 def replay(U0, V0, batches, lr, err_mode, lpr, groups=None):
     """The drain on ``U0`` [n_users, k] and ``V0`` [n_items, k] (float64 holding the fp32 rows) with ``batches`` =
     [(users, items, ratings)] indexing them (``user < 0`` void; ratings as the kernel reads them, so fp16-rounded
@@ -103,7 +77,7 @@ def replay(U0, V0, batches, lr, err_mode, lpr, groups=None):
         groups, attempts = partition([(u, i) for u, i, _ in batches])
     U, V = np.array(U0, dtype=np.float64), np.array(V0, dtype=np.float64)
     tU, tV = np.zeros_like(U), np.zeros_like(V)
-    depth = dot_depth(lpr)
+    depth = dot_depth(-(-U.shape[1] // 4) * 4, lpr)
     lr32 = float(np.float32(lr))
     n = len(batches)
     sq, cnt, tol_sq = np.zeros(n), np.zeros(n), np.zeros(n)
@@ -119,14 +93,14 @@ def replay(U0, V0, batches, lr, err_mode, lpr, groups=None):
                 dd = depth * EPS * np.abs(u0 * v0).sum(1) + (np.abs(u0) * dv0 + np.abs(v0) * du0).sum(1)
                 if singleton:
                     # pushes of the other records to the rows this one pulls, to first order |g| times the row
-                    g0 = _grad(r, d, dd, lr32, err_mode)[2][:, None]
+                    g0 = grad(r, d, dd, lr32, err_mode)[2][:, None]
                     pu, pv = np.abs(g0 * v0), np.abs(g0 * u0)
                     su, sv = np.zeros_like(U), np.zeros_like(V)
                     np.add.at(su, users, pu)
                     np.add.at(sv, items, pv)
                     race_u, race_v = su[users] - pu, sv[items] - pv
                     dd = dd + (np.abs(u0) * race_v + np.abs(v0) * race_u).sum(1)
-                resid, dres, g, dg = _grad(r, d, dd, lr32, err_mode)
+                resid, dres, g, dg = grad(r, d, dd, lr32, err_mode)
                 g, dg = g[:, None], dg[:, None]
                 du_new = np.abs(g) * dv0 + dg * np.abs(v0)
                 dv_new = np.abs(g) * du0 + dg * np.abs(u0)
