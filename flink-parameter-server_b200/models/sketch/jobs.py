@@ -21,7 +21,7 @@ from ...runtime.stream import as_stream
 from ...runtime.transform import (default_param_partitioner, default_worker_partitioner, transform,
                                   transformWithModelLoad)
 from .hashing import floor_mod, hash64, hash64_signed, java_string_hash, murmur3_32
-from .utils import bloomEq, dotProduct, merge_topk
+from .utils import bloomCoOccurrence, dotProduct, java_round, merge_topk
 
 
 def _unsupported(*_a, **_k):
@@ -144,12 +144,11 @@ class BloomPredictPSLogic(ParameterServerLogic):
     def onPushRecv(self, id, deltaUpdate, ps):
         if deltaUpdate.is_left:
             queryId, target = deltaUpdate.value
-            nA = bloomEq(self.m, self.k, len(target))
             topK = []
-            for k, v in self.model.items():
-                nB = bloomEq(self.m, self.k, len(v))
-                union = bloomEq(self.m, self.k, len(target | v))
-                topK.append((nA + nB - union, k))
+            for k, v in self.model.items():     # a saturated union has no estimate: the key is skipped
+                est = bloomCoOccurrence(self.m, self.k, len(target), len(v), len(target | v))
+                if est is not None:
+                    topK.append((est, k))
             ps.output((queryId, sorted(topK)[-self.K:]))
         else:
             self.model[id] = frozenset(deltaUpdate.value)
@@ -266,12 +265,12 @@ class TimeAwareBloomPredictPSLogic(ParameterServerLogic):
     def onPushRecv(self, id, deltaUpdate, ps):
         if deltaUpdate.is_left:
             (queryId, slot), target = deltaUpdate.value
-            nA = bloomEq(self.m, self.k, len(target))
             topK = []
             for (k, s), v in self.model.items():
                 if s == slot:
-                    nB = bloomEq(self.m, self.k, len(v))
-                    topK.append((nA + nB - bloomEq(self.m, self.k, len(target | v)), k))
+                    est = bloomCoOccurrence(self.m, self.k, len(target), len(v), len(target | v))
+                    if est is not None:
+                        topK.append((est, k))
             ps.output(((queryId, slot), sorted(topK)[-self.K:]))
         else:
             slot, bits = deltaUpdate.value
@@ -628,8 +627,9 @@ def word_count(train) -> Dict[int, int]:
 def minhashPredict(words, train, model, numHashes, K, workerParallelism, psParallelism, pullLimit,
                    iterationWaitTime=10000, backend: str = "local", **device_kw):
     """(MinHashPredict.scala:60-141): Jaccard estimates converted to co-occurrence counts with the
-    word frequencies of ``train``: ``round(J * (f_q + f_w) / (J + 1))``; per query the list is
-    sorted by that count, best first."""
+    word frequencies of ``train``: ``java_round(J * (f_q + f_w) / (J + 1))`` in double, evaluated in that
+    order and rounded like Java's ``Math.round`` (halves up, so J = 1 and f_q + f_w = 5 gives 3); per query the
+    list is sorted by that count, best first."""
     if backend == "device":   # Jaccard scan + the Aggregate step (word frequencies) in one kernel
         res = _device_predict("minhash", list(as_stream(words).collect()), model, numHashes, K,
                               counts=word_count(train), cooccurrence=True, **device_kw)
@@ -652,7 +652,7 @@ def minhashPredict(words, train, model, numHashes, K, workerParallelism, psParal
         if count[q] < psParallelism:
             continue
         f = freq.get(q, 0)
-        r = [(w, int(round((v * (f + freq.get(w, 0))) / (v + 1)))) for v, w in inter]
+        r = [(w, java_round((v * (f + freq.get(w, 0))) / (v + 1))) for v, w in inter]
         out.append((q, sorted(r, key=lambda t: t[1], reverse=True)))
     return out
 

@@ -2,7 +2,7 @@
 from __future__ import annotations
 
 import math
-from typing import Iterable, List, Sequence, Tuple
+from typing import Iterable, List, Optional, Sequence, Tuple
 
 
 def dotProduct(u: Sequence[int], v: Sequence[int]) -> int:
@@ -12,6 +12,22 @@ def dotProduct(u: Sequence[int], v: Sequence[int]) -> int:
 def bloomEq(m: float, k: float, size: float) -> float:
     """Cardinality estimate of a Bloom filter with ``size`` set bits: ``-m/k * ln(1 - size/m)``."""
     return -m / k * math.log(1 - size / m)
+
+
+def bloomCoOccurrence(m: float, k: float, sizeA: int, sizeB: int, sizeUnion: int) -> Optional[float]:
+    """``n(A) + n(B) - n(A u B)`` from the set-bit counts, or None when the union has all ``m`` bits set: one of
+    the estimates is then infinite and the score is not a number.  The device scan ranks such a key as not a
+    key (``-3e38``), so both tiers leave it out of the top-K."""
+    if sizeUnion >= m:
+        return None
+    return bloomEq(m, k, sizeA) + bloomEq(m, k, sizeB) - bloomEq(m, k, sizeUnion)
+
+
+def java_round(x: float) -> int:
+    """``Math.round`` on a double: the nearest integer, halves toward +inf.  ``floor(x + 0.5)`` would round
+    0.49999999999999994 up, and Python's ``round`` takes halves to even."""
+    f = math.floor(x)
+    return int(f) + (x - f >= 0.5)
 
 
 def bloomUnion(m: float, k: float, A: Iterable[int], B: Iterable[int]) -> float:

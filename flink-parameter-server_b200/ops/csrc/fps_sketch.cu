@@ -102,10 +102,16 @@ __global__ void __launch_bounds__(256)
       cq += __shfl_xor_sync(0xffffffffu, cq, o);
     }
     if (lane == 0) {
-      const float nA = -m / k * logf(1.f - (float)cq / m);
-      const float nB = -m / k * logf(1.f - (float)cb / m);
-      const float nU = -m / k * logf(1.f - (float)cu / m);
-      est[r] = (cb == 0) ? -3.0e38f : nA + nB - nU;  // empty rows are not keys
+      // bloomEq in fp64, as the reference computes it.  In float, c/m is rounded before 1 - c/m when m is not a
+      // power of two, and at small c that error dominates the log (1% at m = 1000003).  Three logs on one lane
+      // per row, after a popcount pass over the whole row.
+      const double md = m, kd = k;
+      const double nA = -md / kd * log(1.0 - (double)cq / md);
+      const double nB = -md / kd * log(1.0 - (double)cb / md);
+      const double nU = -md / kd * log(1.0 - (double)cu / md);
+      const double e = nA + nB - nU;
+      // empty rows are not keys; a saturated filter makes some n(X) infinite and e NaN or -inf: not a key either
+      est[r] = (cb == 0 || !isfinite(e)) ? -3.0e38f : (float)e;
     }
   }
 }
@@ -128,7 +134,7 @@ extern "C" int fps_bloom_query(const unsigned int* local_rows, long long n_rows,
 // lane g keeps the mean of group g, the median is found by rank counting over shuffles.
 // K10 query: MinHash Jaccard estimate = fraction of signature slots holding the same tweet id
 // (MinHashPredictPSLogic.scala:33-36), optionally converted to a co-occurrence count with the word
-// frequencies, round(J * (f_q + f_w) / (J + 1))  (MinHashPredict.scala:60-141 Aggregate).
+// frequencies, Math.round(J * (f_q + f_w) / (J + 1)) in double  (MinHashPredict.scala:60-141 Aggregate).
 // Time-aware variants (TimeAwareToWPredictPSLogic.scala, TimeAwareBloomPredictPSLogic.scala:19-27): keys
 // are (word, timeSlot); `key_slot[r] != query_slot` rows are excluded from the scan.
 // ----------------------------------------------------------------------------------------
@@ -201,10 +207,20 @@ __global__ void __launch_bounds__(256)
       qfilled += __shfl_xor_sync(0xffffffffu, qfilled, o);
     }
     if (lane == 0) {
-      float j = (filled != 0 && qfilled != 0) ? (float)eq / (float)n_hashes : 0.f;
-      if (filled == 0) j = SK_NEG_INF;                         // not a key of this shard
-      else if (freq != nullptr) j = rintf(j * (query_freq + freq[r]) / (j + 1.f));
-      est[r] = j;
+      const bool both = filled != 0 && qfilled != 0;
+      float s;
+      if (filled == 0) {
+        s = SK_NEG_INF;                                        // not a key of this shard
+      } else if (freq != nullptr) {
+        // Math.round((J * (f_q + f_r)) / (J + 1)) on doubles, in the reference's order: halves round up
+        const double J = both ? (double)eq / (double)n_hashes : 0.0;
+        const double x = J * ((double)query_freq + (double)freq[r]) / (J + 1.0);
+        const double f = floor(x);
+        s = (float)(x - f >= 0.5 ? f + 1.0 : f);
+      } else {
+        s = both ? (float)eq / (float)n_hashes : 0.f;
+      }
+      est[r] = s;
     }
   }
 }

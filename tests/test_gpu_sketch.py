@@ -107,6 +107,7 @@ def test_minhash_jaccard_and_cooccurrence_query_equal_host_predict():
     from fps_b200.models.sketch.device import DeviceSketch
     from fps_b200.models.sketch.hashing import java_string_hash
     from fps_b200.models.sketch.jobs import minhashPredict, word_count
+    from fps_b200.models.sketch.utils import java_round
 
     torch.cuda.set_device(0)
     n = 32
@@ -121,13 +122,14 @@ def test_minhash_jaccard_and_cooccurrence_query_equal_host_predict():
         jac = {k: sum(1 for a, b in zip(v, d[q]) if a == b) / n for k, v in d.items()}
         host_j = sorted(((j, k) for k, j in jac.items()), reverse=True)
         _rank_close(mh.query_local(w, 4), host_j, 4)
-        host_c = sorted(((float(round(j * (freq[q] + freq[k]) / (j + 1))), k) for k, j in jac.items()), reverse=True)
+        host_c = sorted(((float(java_round(j * (freq[q] + freq[k]) / (j + 1))), k) for k, j in jac.items()),
+                        reverse=True)
         _rank_close(mh.query_local(w, 4, cooccurrence=True), host_c, 4)
     mh.close()
     res = dict(minhashPredict(["cat"], TWEETS, model, n, 4, 1, 1, 100, backend="device"))
     q = java_string_hash("cat")
     got = res[q]
-    assert got[0][0] == q and got[0][1] == round(1.0 * (2 * freq[q]) / 2.0)     # J(cat, cat) = 1
+    assert got[0][0] == q and got[0][1] == java_round(1.0 * (2 * freq[q]) / 2.0)     # J(cat, cat) = 1
     assert [c for _, c in got] == sorted((c for _, c in got), reverse=True)
 
 
