@@ -1,5 +1,5 @@
-// word2vec skip-gram from a token stream (DESIGN §2.13): frequent-word subsampling and compaction, then one fused
-// SGNS kernel that trains each kept center over its whole dynamic window.
+// word2vec skip-gram and CBOW from a token stream (DESIGN §2.13, §2.14): frequent-word subsampling and compaction,
+// then one fused SGNS kernel that trains each kept center over its whole dynamic window.
 //
 // Draws, all Philox4x32-10 with counter (c0, c1, c2, c3) and key (seed lo, seed hi), i = the token's position in
 // the call:
@@ -14,17 +14,22 @@
 // each entry's call position in `pos` and its length in *n_comp.  Per-CTA counts, grid sync, CTA offsets, then a
 // ballot scan per CTA writes the entries in order.
 //
-// fps_w2v_window_kernel: one lane-group per compacted entry (grid-stride loop bounded by *n_comp, so the grid is
+// fps_w2v_kernel<CBOW>: one lane-group per compacted entry (grid-stride loop bounded by *n_comp, so the grid is
 // sized without a host sync).  For a kept center c at entry e with radius r, its contexts are the entries
-// e-r .. e+r (not e), stopping at a boundary or the end of the call, visited in increasing position:
-//   u = W_in[c] as pulled, D = 0
-//   per context q: w = u + D, e = 0; targets = (q, label 1), then `negative` noise words (label 0), pulled in
-//     blocks of TB rows; per target: d = w . v_t, g = lr (label - sigmoid(d)), e += g v_t, W_out[t] += g w
-//     (pushed at once);  D += e after the context's targets
-//   W_in[c] += D, pushed once
+// e-r .. e+r (not e), stopping at a boundary or the end of the call, visited in increasing position.  A list of
+// targets is (word, label 1), then `negative` noise words (label 0) rejected against the word, pulled in blocks of
+// TB rows; per target with input w: d = w . v_t, g = lr (label - sigmoid(d)), e += g v_t, W_out[t] += g w (pushed
+// at once).
+//   skip-gram: u = W_in[c] as pulled, D = 0; per context q (slot k): w = u + D, e = 0, the targets of word q,
+//     D += e after them; W_in[c] += D, pushed once
+//   CBOW, for a center with cw >= 1 contexts: h = (sum of W_in[ctx] as pulled, in increasing position) / cw, the
+//     context rows pulled TB at a time before any push; w = h, e = 0, the targets of word c keyed as slot 0;
+//     W_in[ctx] += e for every context, once per occurrence: word2vec.c's mean in, unscaled error out.  A center
+//     with no context trains and counts nothing.
 // A W_out row repeated inside one block of targets is read as it was before the block; one repeated in a later
 // block or context of the same center is read with the earlier pushes applied (the same lanes pushed and pull the
-// same float4s, in program order).  Rows shared between centers are updated Hogwild-style.
+// same float4s, in program order).  Rows shared between centers, W_in rows too under CBOW, are updated
+// Hogwild-style.
 #include <cooperative_groups.h>
 #include <limits.h>
 #include "fps_common.cuh"
@@ -59,7 +64,7 @@ struct W2vArgs {
   float* stats;              // [2] += sum -log sigmoid(+-d), targets trained
   int* nan_flag;
   int reserve_total;         // CTA slots left free for the replica exchange
-  int pad_;
+  int cbow;                  // 0 = skip-gram, 1 = CBOW
 };
 
 __device__ __forceinline__ unsigned long long w2v_hash(const W2vArgs& a, long long i, uint32_t c1, uint32_t c2) {
@@ -229,8 +234,8 @@ __device__ __forceinline__ float4 w2v_add4(float4 a, float4 b) {
 }
 __device__ __forceinline__ float w2v_dot4(float4 w, float4 v) { return w.x * v.x + w.y * v.y + w.z * v.z + w.w * v.w; }
 
-template <int LPR, int VPL, int MINB, int TB>
-__global__ void __launch_bounds__(W2V_THREADS, MINB) fps_w2v_window_kernel(const __grid_constant__ W2vArgs a) {
+template <bool CBOW, int LPR, int VPL, int MINB, int TB>
+__global__ void __launch_bounds__(W2V_THREADS, MINB) fps_w2v_kernel(const __grid_constant__ W2vArgs a) {
   const int lane = threadIdx.x & (LPR - 1);
   const long long group = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LPR;
   const long long n_groups = ((long long)gridDim.x * blockDim.x) / LPR;
@@ -255,25 +260,63 @@ __global__ void __launch_bounds__(W2V_THREADS, MINB) fps_w2v_window_kernel(const
     }
     const int n_left = (int)(e - L), n_ctx = (int)(R - L);
     float* up = fps_row32(a.w_in, ok ? center : 0);
-    float4 u[VPL], D[VPL];
+    float4 u[VPL], D[VPL];    // skip-gram: u and D
+    float4 h[VPL], ev[VPL];   // CBOW: h; both: e of the current targets
+    if constexpr (!CBOW) {
 #pragma unroll
-    for (int c = 0; c < VPL; ++c) {
-      const int q = lane + c * LPR;
-      u[c] = (ok && q < nvec) ? fps_ld_row4(up + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);   // the PULL of u
-      D[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int c = 0; c < VPL; ++c) {
+        const int q = lane + c * LPR;
+        u[c] = (ok && q < nvec) ? fps_ld_row4(up + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);   // the PULL of u
+        D[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    } else {
+      const bool has_ctx = n_ctx > 0;   // tested before the pulls, for the code nvcc makes (NOTES, Pitfalls)
+#pragma unroll
+      for (int c = 0; c < VPL; ++c) {
+        h[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+        ev[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      // the PULL of the context rows, TB in flight at a time, summed in increasing position
+      for (int k0 = 0; k0 < n_ctx; k0 += TB) {
+        float4 x[TB][VPL];
+#pragma unroll
+        for (int b = 0; b < TB; ++b) {
+          const int k = k0 + b;
+          const int ctx = k < n_ctx ? a.seq[k < n_left ? L + k : e + 1 + (k - n_left)] : -1;
+          const float* xp = fps_row32(a.w_in, ctx >= 0 ? ctx : 0);
+#pragma unroll
+          for (int c = 0; c < VPL; ++c) {
+            const int q = lane + c * LPR;
+            x[b][c] = (ctx >= 0 && q < nvec) ? fps_ld_row4(xp + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
+          }
+        }
+#pragma unroll
+        for (int b = 0; b < TB; ++b) {
+          if (k0 + b >= n_ctx) break;
+#pragma unroll
+          for (int c = 0; c < VPL; ++c) h[c] = w2v_add4(h[c], x[b][c]);
+        }
+      }
+      if (has_ctx) {
+        const float cw = (float)n_ctx;
+#pragma unroll
+        for (int c = 0; c < VPL; ++c) h[c] = make_float4(h[c].x / cw, h[c].y / cw, h[c].z / cw, h[c].w / cw);
+      }
     }
-    for (int k = 0; __any_sync(0xffffffffu, k < n_ctx); ++k) {
+    // one list of targets per context (skip-gram) or one per center, keyed as context slot 0 (CBOW)
+    for (int k = 0; CBOW ? k == 0 : __any_sync(0xffffffffu, k < n_ctx); ++k) {
       const bool live = k < n_ctx;
-      int ctx = -1;
-      if (live) ctx = a.seq[k < n_left ? L + k : e + 1 + (k - n_left)];
-      float4 ev[VPL];
+      int word = CBOW ? center : -1;   // the label-1 target, which the noise words must differ from
+      if (!CBOW && live) word = a.seq[k < n_left ? L + k : e + 1 + (k - n_left)];
+      if constexpr (!CBOW) {
 #pragma unroll
-      for (int c = 0; c < VPL; ++c) ev[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-      // the context's noise words: with negative <= LPR, lane l of the group draws negative l, so the draws (a
-      // binary search of the CDF each) run side by side instead of one after another
+        for (int c = 0; c < VPL; ++c) ev[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      // with negative <= LPR, lane l of the group draws negative l, so the draws (a binary search of the CDF each)
+      // run side by side instead of one after another
       const bool par = a.negative <= LPR;
       int mine = -1;
-      if (par && live && lane < a.negative) mine = w2v_negative(a, i, k, lane, ctx);
+      if (par && live && lane < a.negative) mine = w2v_negative(a, i, k, lane, word);
       for (int t0 = 0; t0 < T; t0 += TB) {
         int tid[TB];
         float4 v[TB][VPL];
@@ -283,7 +326,7 @@ __global__ void __launch_bounds__(W2V_THREADS, MINB) fps_w2v_window_kernel(const
           const int src = (int)(threadIdx.x & 31 & ~(LPR - 1)) + (t >= 1 && t - 1 < LPR ? t - 1 : 0);
           const int drawn = __shfl_sync(0xffffffffu, mine, src);
           int id = -1;
-          if (live && t < T) id = t == 0 ? ctx : par ? drawn : w2v_negative(a, i, k, t - 1, ctx);
+          if (live && t < T) id = t == 0 ? word : par ? drawn : w2v_negative(a, i, k, t - 1, word);
           tid[b] = id;
           const float* vp = fps_row32(a.w_out, id >= 0 ? id : 0);
 #pragma unroll
@@ -297,7 +340,7 @@ __global__ void __launch_bounds__(W2V_THREADS, MINB) fps_w2v_window_kernel(const
           if (t0 + b >= T) break;           // uniform: T is the same for every group
           float part = 0.f;
 #pragma unroll
-          for (int c = 0; c < VPL; ++c) part += w2v_dot4(w2v_add4(u[c], D[c]), v[b][c]);
+          for (int c = 0; c < VPL; ++c) part += w2v_dot4(CBOW ? h[c] : w2v_add4(u[c], D[c]), v[b][c]);
           const float d = fps_group_sum<LPR>(part);
           if (tid[b] < 0) continue;
           if (!(fabsf(d) <= 3.0e38f)) bad = true;   // NaN/Inf guard
@@ -315,170 +358,45 @@ __global__ void __launch_bounds__(W2V_THREADS, MINB) fps_w2v_window_kernel(const
             if (q < nvec) {
               ev[c].x += g * v[b][c].x; ev[c].y += g * v[b][c].y;
               ev[c].z += g * v[b][c].z; ev[c].w += g * v[b][c].w;
-              const float4 w = w2v_add4(u[c], D[c]);
-              fps_red_add4(vp + 4 * q, make_float4(g * w.x, g * w.y, g * w.z, g * w.w));   // the PUSH of g (u + D)
+              // CBOW reads h[c] in place: a copy of it changes the code nvcc makes at VPL = 1
+              float4 s;
+              if constexpr (!CBOW) s = w2v_add4(u[c], D[c]);
+              const float4& w = CBOW ? h[c] : s;
+              fps_red_add4(vp + 4 * q, make_float4(g * w.x, g * w.y, g * w.z, g * w.w));   // the PUSH of g w
             }
           }
         }
       }
-      if (live) {
+      if constexpr (!CBOW) {
+        if (live) {
 #pragma unroll
-        for (int c = 0; c < VPL; ++c) {
-          D[c].x += ev[c].x; D[c].y += ev[c].y; D[c].z += ev[c].z; D[c].w += ev[c].w;
-        }
-        if (lane == 0) ++ctx_acc;
-      }
-    }
-    if (ok) {
-#pragma unroll
-      for (int c = 0; c < VPL; ++c) {
-        const int q = lane + c * LPR;
-        if (q < nvec) fps_red_add4(up + 4 * q, D[c]);   // the one PUSH of the center row
-      }
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    loss_acc += __shfl_xor_sync(0xffffffffu, loss_acc, o);
-    tgt_acc += __shfl_xor_sync(0xffffffffu, tgt_acc, o);
-    ctx_acc += __shfl_xor_sync(0xffffffffu, ctx_acc, o);
-  }
-  if ((threadIdx.x & 31) == 0 && tgt_acc > 0.f) {
-    if (a.stats != nullptr) {
-      atomicAdd(a.stats + 0, loss_acc);
-      atomicAdd(a.stats + 1, tgt_acc);
-    }
-    if (a.token_stats != nullptr) atomicAdd((unsigned long long*)a.token_stats + 2, ctx_acc);
-  }
-  if (bad && a.nan_flag != nullptr) *a.nan_flag = 1;
-}
-
-// fps_w2v_cbow_kernel (DESIGN §2.14): the entries, windows and draws of the skip-gram kernel, but one target list
-// per center.  For a kept center c at call position i with cw >= 1 contexts:
-//   h = (sum of W_in[ctx] as pulled, in increasing position) / cw, e = 0
-//   targets = (c, label 1), then `negative` noise words drawn as those of context slot 0 but rejected against c,
-//     pulled in blocks of TB rows; per target: d = h . v_t, g = lr (label - sigmoid(d)), e += g v_t,
-//     W_out[t] += g h (pushed at once)
-//   W_in[ctx] += e for every context, once per occurrence: word2vec.c's mean in, unscaled error out
-// The context rows are pulled TB at a time, all of them before any push of the center.  A center with no context
-// trains and counts nothing.  Neighbouring centers read and push the same W_in rows, Hogwild-style.
-template <int LPR, int VPL, int MINB, int TB>
-__global__ void __launch_bounds__(W2V_THREADS, MINB) fps_w2v_cbow_kernel(const __grid_constant__ W2vArgs a) {
-  const int lane = threadIdx.x & (LPR - 1);
-  const long long group = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LPR;
-  const long long n_groups = ((long long)gridDim.x * blockDim.x) / LPR;
-  const int nvec = a.stride >> 2;
-  const int T = 1 + a.negative;
-  const long long n = *a.n_comp;
-  float loss_acc = 0.f, tgt_acc = 0.f;
-  unsigned long long ctx_acc = 0;
-  bool bad = false;
-
-  // the trip count is the same for every lane of a warp (n_groups is a multiple of 32 / LPR)
-  const long long n_round = ((n + n_groups - 1) / n_groups) * n_groups;
-  for (long long e = group; e < n_round; e += n_groups) {
-    const int center = e < n ? a.seq[e] : -1;
-    long long i = 0, L = e, R = e;
-    if (center >= 0) {
-      i = a.pos[e];
-      const long long r = 1 + (long long)(w2v_hash(a, i, 1u, 0u) % (unsigned long long)a.window);
-      for (long long q = e - 1; q >= e - r && q >= 0 && a.seq[q] >= 0; --q) L = q;
-      for (long long q = e + 1; q <= e + r && q < n && a.seq[q] >= 0; ++q) R = q;
-    }
-    const int n_left = (int)(e - L), n_ctx = (int)(R - L);
-    const bool live = n_ctx > 0;   // a kept center with at least one context
-    float4 h[VPL], ev[VPL];
-#pragma unroll
-    for (int c = 0; c < VPL; ++c) {
-      h[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-      ev[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    // the PULL of the context rows, TB in flight at a time, summed in increasing position
-    for (int k0 = 0; k0 < n_ctx; k0 += TB) {
-      float4 x[TB][VPL];
-#pragma unroll
-      for (int b = 0; b < TB; ++b) {
-        const int k = k0 + b;
-        const int ctx = k < n_ctx ? a.seq[k < n_left ? L + k : e + 1 + (k - n_left)] : -1;
-        const float* xp = fps_row32(a.w_in, ctx >= 0 ? ctx : 0);
-#pragma unroll
-        for (int c = 0; c < VPL; ++c) {
-          const int q = lane + c * LPR;
-          x[b][c] = (ctx >= 0 && q < nvec) ? fps_ld_row4(xp + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-#pragma unroll
-      for (int b = 0; b < TB; ++b) {
-        if (k0 + b >= n_ctx) break;
-#pragma unroll
-        for (int c = 0; c < VPL; ++c) h[c] = w2v_add4(h[c], x[b][c]);
-      }
-    }
-    if (live) {
-      const float cw = (float)n_ctx;
-#pragma unroll
-      for (int c = 0; c < VPL; ++c) h[c] = make_float4(h[c].x / cw, h[c].y / cw, h[c].z / cw, h[c].w / cw);
-    }
-    // the center's noise words, keyed as context slot 0: with negative <= LPR lane l of the group draws word l
-    const bool par = a.negative <= LPR;
-    int mine = -1;
-    if (par && live && lane < a.negative) mine = w2v_negative(a, i, 0, lane, center);
-    for (int t0 = 0; t0 < T; t0 += TB) {
-      int tid[TB];
-      float4 v[TB][VPL];
-#pragma unroll
-      for (int b = 0; b < TB; ++b) {   // the block's ids, then all of its pulls
-        const int t = t0 + b;
-        const int src = (int)(threadIdx.x & 31 & ~(LPR - 1)) + (t >= 1 && t - 1 < LPR ? t - 1 : 0);
-        const int drawn = __shfl_sync(0xffffffffu, mine, src);
-        int id = -1;
-        if (live && t < T) id = t == 0 ? center : par ? drawn : w2v_negative(a, i, 0, t - 1, center);
-        tid[b] = id;
-        const float* vp = fps_row32(a.w_out, id >= 0 ? id : 0);
-#pragma unroll
-        for (int c = 0; c < VPL; ++c) {
-          const int q = lane + c * LPR;
-          v[b][c] = (id >= 0 && q < nvec) ? fps_ld_row4(vp + 4 * q) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-#pragma unroll
-      for (int b = 0; b < TB; ++b) {
-        if (t0 + b >= T) break;           // uniform: T is the same for every group
-        float part = 0.f;
-#pragma unroll
-        for (int c = 0; c < VPL; ++c) part += w2v_dot4(h[c], v[b][c]);
-        const float d = fps_group_sum<LPR>(part);
-        if (tid[b] < 0) continue;
-        if (!(fabsf(d) <= 3.0e38f)) bad = true;   // NaN/Inf guard
-        const float label = (t0 + b == 0) ? 1.f : 0.f;
-        const float g = a.lr * (label - 1.f / (1.f + __expf(-d)));
-        if (lane == 0) {
-          const float x = (t0 + b == 0) ? -d : d;   // -log sigmoid(+-d) = softplus(-+d)
-          loss_acc += fmaxf(x, 0.f) + log1pf(__expf(-fabsf(x)));
-          tgt_acc += 1.f;
-        }
-        float* vp = fps_row32(a.w_out, tid[b]);
-#pragma unroll
-        for (int c = 0; c < VPL; ++c) {
-          const int q = lane + c * LPR;
-          if (q < nvec) {
-            ev[c].x += g * v[b][c].x; ev[c].y += g * v[b][c].y;
-            ev[c].z += g * v[b][c].z; ev[c].w += g * v[b][c].w;
-            fps_red_add4(vp + 4 * q, make_float4(g * h[c].x, g * h[c].y, g * h[c].z, g * h[c].w));   // PUSH g h
+          for (int c = 0; c < VPL; ++c) {
+            D[c].x += ev[c].x; D[c].y += ev[c].y; D[c].z += ev[c].z; D[c].w += ev[c].w;
           }
+          if (lane == 0) ++ctx_acc;
         }
       }
     }
-    // the PUSH of e to every context row, once per occurrence
-    for (int k = 0; k < n_ctx; ++k) {
-      float* xp = fps_row32(a.w_in, a.seq[k < n_left ? L + k : e + 1 + (k - n_left)]);
+    if constexpr (!CBOW) {
+      if (ok) {
 #pragma unroll
-      for (int c = 0; c < VPL; ++c) {
-        const int q = lane + c * LPR;
-        if (q < nvec) fps_red_add4(xp + 4 * q, ev[c]);
+        for (int c = 0; c < VPL; ++c) {
+          const int q = lane + c * LPR;
+          if (q < nvec) fps_red_add4(up + 4 * q, D[c]);   // the one PUSH of the center row
+        }
       }
+    } else {
+      // the PUSH of e to every context row, once per occurrence
+      for (int k = 0; k < n_ctx; ++k) {
+        float* xp = fps_row32(a.w_in, a.seq[k < n_left ? L + k : e + 1 + (k - n_left)]);
+#pragma unroll
+        for (int c = 0; c < VPL; ++c) {
+          const int q = lane + c * LPR;
+          if (q < nvec) fps_red_add4(xp + 4 * q, ev[c]);
+        }
+      }
+      if (lane == 0) ctx_acc += (unsigned long long)n_ctx;
     }
-    if (lane == 0) ctx_acc += (unsigned long long)n_ctx;
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -499,9 +417,9 @@ __global__ void __launch_bounds__(W2V_THREADS, MINB) fps_w2v_cbow_kernel(const _
 // One CTA per SM slot the occupancy allows, less `reserve_total` for the replica exchange; the grid-stride loop
 // covers however many entries the subsample kernel wrote, so the grid needs no host-side count.
 template <int LPR, int VPL, int MINB, int TB>
-static int launch_w2v(const W2vArgs& a, bool cbow, int num_sms, cudaStream_t stream) {
-  void (*kern)(const W2vArgs) = cbow ? fps_w2v_cbow_kernel<LPR, VPL, MINB, TB>
-                                     : fps_w2v_window_kernel<LPR, VPL, MINB, TB>;
+static int launch_w2v(const W2vArgs& a, int num_sms, cudaStream_t stream) {
+  void (*kern)(const W2vArgs) = a.cbow ? fps_w2v_kernel<true, LPR, VPL, MINB, TB>
+                                       : fps_w2v_kernel<false, LPR, VPL, MINB, TB>;
   const long long blocks = fps_row_grid(kern, W2V_THREADS, W2V_THREADS / LPR, num_sms, a.reserve_total, 0, 1,
                                         a.n_tokens, 1);   // n_comp <= n_tokens
   kern<<<(int)blocks, W2V_THREADS, 0, stream>>>(a);
@@ -509,32 +427,24 @@ static int launch_w2v(const W2vArgs& a, bool cbow, int num_sms, cudaStream_t str
 }
 
 // Lane geometry of dispatch_bpr: LPR lanes per row, VPL float4 per lane; MINB keeps each free of spills (ptxas -v).
-// TB target rows are pulled at once: 8 (every target of a context while negative <= 7), 6 for rows over 384 floats,
-// where 8 rows of 4 float4 per lane do not fit in 255 registers (6 = word2vec's default negative = 5).
-static int w2v_dispatch(const W2vArgs& a, bool cbow, int num_sms, cudaStream_t stream) {
+// TB target rows, and under CBOW TB context rows, are pulled at once: 8 (every target of a context while
+// negative <= 7), 6 for rows over 384 floats, where 8 rows of 4 float4 per lane do not fit in 255 registers (6 =
+// word2vec's default negative = 5).
+extern "C" int fps_w2v_window_fused(const W2vArgs* args, int num_sms, cudaStream_t stream) {
+  const W2vArgs& a = *args;
   if (a.n_tokens <= 0) return 0;
   if ((a.stride & 3) != 0 || a.window < 1 || a.window >= (1 << 23) || a.negative < 0 || a.negative > 255 ||
-      a.max_tries < 1 || a.max_tries >= (1 << 23) || a.vocab < 1 || a.vocab > INT_MAX)
+      a.max_tries < 1 || a.max_tries >= (1 << 23) || a.vocab < 1 || a.vocab > INT_MAX || (a.cbow & ~1) != 0)
     return -1501;
   const int nvec = a.stride >> 2;
-  if (nvec <= 1) return launch_w2v<1, 1, 2, 8>(a, cbow, num_sms, stream);
-  if (nvec <= 2) return launch_w2v<2, 1, 2, 8>(a, cbow, num_sms, stream);
-  if (nvec <= 4) return launch_w2v<4, 1, 2, 8>(a, cbow, num_sms, stream);
-  if (nvec <= 8) return launch_w2v<8, 1, 2, 8>(a, cbow, num_sms, stream);
-  if (nvec <= 16) return launch_w2v<16, 1, 2, 8>(a, cbow, num_sms, stream);
-  if (nvec <= 32) return launch_w2v<32, 1, 2, 8>(a, cbow, num_sms, stream);
-  if (nvec <= 64) return launch_w2v<32, 2, 1, 8>(a, cbow, num_sms, stream);
-  if (nvec <= 96) return launch_w2v<32, 3, 1, 8>(a, cbow, num_sms, stream);
-  if (nvec <= 128) return launch_w2v<32, 4, 1, 6>(a, cbow, num_sms, stream);
+  if (nvec <= 1) return launch_w2v<1, 1, 2, 8>(a, num_sms, stream);
+  if (nvec <= 2) return launch_w2v<2, 1, 2, 8>(a, num_sms, stream);
+  if (nvec <= 4) return launch_w2v<4, 1, 2, 8>(a, num_sms, stream);
+  if (nvec <= 8) return launch_w2v<8, 1, 2, 8>(a, num_sms, stream);
+  if (nvec <= 16) return launch_w2v<16, 1, 2, 8>(a, num_sms, stream);
+  if (nvec <= 32) return launch_w2v<32, 1, 2, 8>(a, num_sms, stream);
+  if (nvec <= 64) return launch_w2v<32, 2, 1, 8>(a, num_sms, stream);
+  if (nvec <= 96) return launch_w2v<32, 3, 1, 8>(a, num_sms, stream);
+  if (nvec <= 128) return launch_w2v<32, 4, 1, 6>(a, num_sms, stream);
   return -1000;   // rows wider than 512 floats
-}
-
-extern "C" int fps_w2v_window_fused(const W2vArgs* args, int num_sms, cudaStream_t stream) {
-  return w2v_dispatch(*args, false, num_sms, stream);
-}
-
-// CBOW (DESIGN §2.14): the same argument checks and lane geometry; TB is also the number of context rows pulled at
-// once.
-extern "C" int fps_w2v_cbow_fused(const W2vArgs* args, int num_sms, cudaStream_t stream) {
-  return w2v_dispatch(*args, true, num_sms, stream);
 }

@@ -819,7 +819,7 @@ class W2vArgsC(C.Structure):
         ("w_in", ShardTableC), ("w_out", ShardTableC),
         ("window", C.c_int), ("negative", C.c_int), ("max_tries", C.c_int), ("lr", C.c_float),
         ("cdf", C.c_void_p), ("last_nonzero", C.c_longlong), ("stats", C.c_void_p), ("nan_flag", C.c_void_p),
-        ("reserve_total", C.c_int), ("pad_", C.c_int),
+        ("reserve_total", C.c_int), ("cbow", C.c_int),
     ]
 
 
@@ -888,7 +888,7 @@ def w2v_window_fused(seq: torch.Tensor, pos: torch.Tensor, n_comp: torch.Tensor,
                      reserve_total: int = 0, cbow: bool = False) -> None:
     """Fused center-window skip-gram negative-sampling step (csrc/fps_w2v_window.cu, DESIGN §2.13) over the
     compacted sequence of :func:`w2v_subsample`; one lane-group per kept center, the grid sized without reading
-    ``n_comp`` on the host.  ``cbow=True`` runs the CBOW kernel instead (DESIGN §2.14), described below.
+    ``n_comp`` on the host.  ``cbow=True`` trains CBOW instead (DESIGN §2.14), described below.
 
     The center at call position ``i`` draws a radius ``r = 1 + h mod window`` (``h`` keyed ``(i, 1, 0, step)``);
     its contexts are the entries up to ``r`` positions to either side, stopping at a boundary, in increasing
@@ -943,11 +943,8 @@ def w2v_window_fused(seq: torch.Tensor, pos: torch.Tensor, n_comp: torch.Tensor,
     if nan_flag is not None:
         _req(nan_flag, "nan_flag", torch.int32)
         a.nan_flag = nan_flag.data_ptr()
-    a.reserve_total = int(reserve_total)
-    if cbow:
-        _check(lib().fps_w2v_cbow_fused(C.byref(a), sm_count(seq.device.index), _stream()), "w2v_cbow_fused")
-    else:
-        _check(lib().fps_w2v_window_fused(C.byref(a), sm_count(seq.device.index), _stream()), "w2v_window_fused")
+    a.reserve_total, a.cbow = int(reserve_total), int(cbow)
+    _check(lib().fps_w2v_window_fused(C.byref(a), sm_count(seq.device.index), _stream()), "w2v_window_fused")
     _bump()
 
 

@@ -1,7 +1,7 @@
-"""The fused CBOW kernel (``fps_w2v_cbow_kernel``, ``train_tokens(cbow=True)``) against the fp64 replay of
-``models/w2v_ref.py``, every Philox draw replayed by ``tests/philox_ref.py``: every dispatch rung and noise path,
-the mean over up to ``2 * window`` contexts, repeated and voided rows, a realistic corpus, grid-stride rounds, the
-ends of a call, the counters, no host sync, the quality it reaches and the 2-rank check."""
+"""The fused window kernel's CBOW (``fps_w2v_kernel<true, ...>``, ``train_tokens(cbow=True)``) against the fp64
+replay of ``models/w2v_ref.py``, every Philox draw replayed by ``tests/philox_ref.py``: every dispatch rung and noise
+path, the mean over up to ``2 * window`` contexts, repeated and voided rows, a realistic corpus, grid-stride rounds,
+the ends of a call, the counters, no host sync, the quality it reaches and the 2-rank check."""
 import functools
 
 import numpy as np
@@ -12,24 +12,9 @@ import fps_b200  # noqa: F401
 from fps_b200.models import w2v_ref as R
 from fps_b200.ops import native
 from tests.philox_ref import philox4x32 as PH
+from tests.w2v_cases import ATOL_OF_MAX, RTOL, RUNGS, SEED, SWEEP, VOCAB, close, fused, noise_dist, tables
 
 pytestmark = pytest.mark.gpu
-
-SEED = 4
-
-# The dispatch ladder is the skip-gram kernel's (tests/test_gpu_w2v_window_edges.py): dim -> (LPR, VPL, TB).
-RUNGS = {3: (1, 1, 8), 4: (1, 1, 8), 8: (2, 1, 8), 13: (4, 1, 8), 16: (4, 1, 8), 24: (8, 1, 8), 36: (16, 1, 8),
-         100: (32, 1, 8), 136: (32, 2, 8), 256: (32, 2, 8), 300: (32, 3, 8), 387: (32, 4, 6), 388: (32, 4, 6),
-         512: (32, 4, 6)}
-SWEEP = [(dim, neg) for dim, (lpr, _, _) in RUNGS.items() for neg in sorted({0, 1, lpr, lpr + 1, 7, 8, 20})]
-
-# The fp32 kernel against the fp64 replay: the tolerance of the skip-gram edge tests.
-RTOL, ATOL_OF_MAX = 2e-5, 1e-5
-
-
-def _close(got, want, what):
-    np.testing.assert_allclose(got, want, rtol=RTOL, atol=ATOL_OF_MAX * float(np.abs(want).max()), err_msg=what)
-
 
 @pytest.fixture
 def dev():
@@ -43,34 +28,6 @@ def test_sweep_reaches_every_rung_and_noise_path():
     paths = {("shuffled" if n <= RUNGS[d][0] else "serial", "one block" if 1 + n <= RUNGS[d][2] else "several")
              for d, n in SWEEP}
     assert paths == {(a, b) for a in ("shuffled", "serial") for b in ("one block", "several")}
-
-
-def _tables(vocab, dim, scale, seed, dev):
-    """W_in and W_out ``[vocab, stride]`` fp32, uniform on +-scale, padding columns 0."""
-    g = torch.Generator(device=dev).manual_seed(seed)
-    out = []
-    for _ in range(2):
-        t = torch.zeros(vocab, (dim + 3) // 4 * 4, device=dev)
-        t[:, :dim] = (torch.rand(vocab, dim, generator=g, device=dev) * 2 - 1) * scale
-        out.append(t)
-    return out
-
-
-def _fused(W_in, W_out, dim, tokens, vocab, *, lr, window, neg, step=0, max_tries=32, cdf=None, last=0,
-           keep_p=None, reserve=0):
-    """One CBOW call through native.w2v_subsample + native.w2v_window_fused(cbow=True); returns (stats,
-    token_stats, nan_flag)."""
-    dev = W_in.device
-    st = torch.zeros(2, dtype=torch.float32, device=dev)
-    ts = torch.zeros(4, dtype=torch.int64, device=dev)
-    nan = torch.zeros(1, dtype=torch.int32, device=dev)
-    seq, pos, n_comp = native.w2v_subsample(tokens, vocab, keep_p, seed=SEED, step=step, token_stats=ts)
-    native.w2v_window_fused(seq, pos, n_comp, native.local_table(W_in, dim), native.local_table(W_out, dim), lr,
-                            window=window, negative=neg, vocab=vocab, seed=SEED, step=step, cdf=cdf,
-                            last_nonzero=last, max_tries=max_tries, stats=st, token_stats=ts, nan_flag=nan,
-                            reserve_total=reserve, cbow=True)
-    torch.cuda.synchronize()
-    return st.cpu(), ts.cpu(), int(nan.item())
 
 
 def _plan(tok, vocab, window, neg, step=0, **noise):
@@ -102,28 +59,12 @@ def _untouched_equal(got, before, rows, vocab):
 
 # ---- every rung x every noise path: sentences `x y`, no row read by two centers --------------------------------
 
-VOCAB = 100_000
-
-
-@functools.lru_cache(maxsize=None)
-def _noise(kind):
-    """(counts, cdf, last_nonzero) of the unigram noise: 30% of the words and the last 1000 have weight 0."""
-    if kind == "uniform":
-        return None, None, 0
-    g = np.random.default_rng(11)
-    c = g.integers(1, 50, size=VOCAB).astype(np.float64)
-    c[g.random(VOCAB) < 0.3] = 0.0
-    c[-1000:] = 0.0
-    cdf = native.noise_cdf(torch.from_numpy(c).cuda(), 0.75).cpu().numpy()
-    return c, cdf, int(np.flatnonzero(c)[-1])
-
-
 @functools.lru_cache(maxsize=None)
 def _pair_corpus(neg, kind, n_sent=16):
     """Sentences ``x y -1`` whose centers pull pairwise disjoint W_out rows.  The center x reads only W_in[y], which
     only x pushes to (after its pull), so nothing depends on the order the lane-groups run in.  A candidate
     sentence that would read a row another center reads is replaced by a boundary."""
-    _, cdf, last = _noise(kind)
+    _, cdf, last = noise_dist(kind)
     words = iter(np.random.default_rng(100 + neg).permutation(VOCAB).tolist())
     tok, used, n_ok = [], set(), 0
     while n_ok < n_sent:
@@ -147,20 +88,20 @@ def test_cbow_kernel_matches_fp64_replay_at_every_rung(dev, dim, neg, noise):
     from fps_b200.models.w2v import DeviceSkipGram
 
     lr = 0.1
-    counts, cdf, last = _noise(noise)
+    counts, cdf, last = noise_dist(noise)
     tok = _pair_corpus(neg, noise)
     plan = _plan(tok, VOCAB, 5, neg, cdf=cdf, last_nonzero=last)
     m = DeviceSkipGram(VOCAB, dim, learning_rate=lr, negative=neg, seed=SEED, noise_counts=counts, sample=0.0)
     try:
-        W_in, W_out = _tables(VOCAB, dim, dim ** -0.25, dim + neg, dev)
+        W_in, W_out = tables(VOCAB, dim, dim ** -0.25, dim + neg, dev)
         m.w_in.local.copy_(W_in)
         m.w_out.local.copy_(W_out)
         rin, w_in, rout, w_out, loss = _replay(W_in, W_out, dim, plan, lr)
         m.train_tokens(torch.from_numpy(tok).to(dev), window=5, cbow=True)
         torch.cuda.synchronize()
         got_in, got_out = m.w_in.local, m.w_out.local
-        _close(got_in[rin, :dim].cpu().numpy(), w_in, "W_in")
-        _close(got_out[rout, :dim].cpu().numpy(), w_out, "W_out")
+        close(got_in[rin, :dim].cpu().numpy(), w_in, "W_in")
+        close(got_out[rout, :dim].cpu().numpy(), w_out, "W_out")
         assert _untouched_equal(got_in, W_in, rin, VOCAB) and _untouched_equal(got_out, W_out, rout, VOCAB)
         assert not got_in[:, dim:].any() and not got_out[:, dim:].any()
         n_centers = int((tok >= 0).sum())
@@ -208,7 +149,7 @@ def test_mean_over_many_contexts_matches_replay_exactly(dev, dim, neg):
     window, lr = 5, 0.1
     tok, plan, chosen = _long_corpus(neg, window, 14, 6, dim + neg)
     assert max(len(plan[k][0]) for k in chosen) == 2 * window
-    W_in, _ = _tables(VOCAB, dim, 0.5, dim, dev)
+    W_in, _ = tables(VOCAB, dim, 0.5, dim, dev)
     W_out = torch.zeros_like(W_in)
     hot = sorted({t for k in chosen for t, _ in plan[k][1]})
     W_out[hot, :dim] = (torch.rand(len(hot), dim, device=dev) * 2 - 1) * 0.5
@@ -216,11 +157,11 @@ def test_mean_over_many_contexts_matches_replay_exactly(dev, dim, neg):
     _, w_in_r, _, w_out_r, _ = _replay(W_in, W_out, dim, plan, lr, order="reverse")
     np.testing.assert_allclose(w_in_r, w_in, rtol=1e-12, atol=1e-15)
     a, b = W_in.clone(), W_out.clone()
-    st, ts, nan = _fused(a, b, dim, torch.from_numpy(tok).to(dev), VOCAB, lr=lr, window=window, neg=neg)
-    _close(a[rin, :dim].cpu().numpy(), w_in, "W_in")
+    st, ts, nan = fused(a, b, dim, torch.from_numpy(tok).to(dev), VOCAB, lr=lr, window=window, neg=neg, cbow=True)
+    close(a[rin, :dim].cpu().numpy(), w_in, "W_in")
     got_out = b[rout, :dim].cpu().numpy()
     is_hot = np.isin(rout, hot)
-    _close(got_out[is_hot], w_out[is_hot], "designated W_out")
+    close(got_out[is_hot], w_out[is_hot], "designated W_out")
     lo, hi = np.minimum(w_out, w_out_r)[~is_hot], np.maximum(w_out, w_out_r)[~is_hot]
     tol = RTOL * np.abs(hi) + ATOL_OF_MAX * float(np.abs(w_out).max())
     assert ((got_out[~is_hot] >= lo - tol) & (got_out[~is_hot] <= hi + tol)).all(), "other W_out"
@@ -250,18 +191,18 @@ def test_void_and_repeated_targets_match_fp64_replay(dev, dim, neg, max_tries, n
     noise_kw = dict(cdf=cdf, last_nonzero=last, max_tries=max_tries)
     seen = set()
     for step in range(2 if neg == 255 else 6):
-        W_in, W_out = _tables(vocab, dim, 0.5, step, dev)
+        W_in, W_out = tables(vocab, dim, 0.5, step, dev)
         W_in[y] = 0.0
         in0 = W_in.cpu().numpy()
         w_in, w_out = W_in[:, :dim].double().cpu().numpy(), W_out[:, :dim].double().cpu().numpy()
         h_y = w_in[x].copy()
         want = R.train_call(w_in, w_out, [x, y], lr=lr, window=5, negative_count=neg, step=step, seed=SEED,
                             philox=PH, cbow=True, **noise_kw)
-        st, ts, nan = _fused(W_in, W_out, dim, tokens, vocab, lr=lr, window=5, neg=neg, step=step,
-                             max_tries=max_tries, cdf=cdf_d, last=last)
+        st, ts, nan = fused(W_in, W_out, dim, tokens, vocab, lr=lr, window=5, neg=neg, step=step,
+                            max_tries=max_tries, cdf=cdf_d, last=last, cbow=True)
         got_in, got_out = W_in.cpu().numpy(), W_out.cpu().numpy()
-        _close(got_out[:, :dim], w_out, f"W_out, step {step}")
-        _close(got_in[x, :dim], w_in[x], f"W_in[x], step {step}")
+        close(got_out[:, :dim], w_out, f"W_out, step {step}")
+        close(got_in[x, :dim], w_in[x], f"W_in[x], step {step}")
         sx = [t for t, _ in R.center_targets(0, [x], neg, vocab, step, SEED, PH, **noise_kw)[0]]
         sy = [t for t, _ in R.center_targets(1, [y], neg, vocab, step, SEED, PH, **noise_kw)[0]]
         assert x not in sx[1:] and y not in sy[1:]
@@ -312,10 +253,11 @@ def test_repeated_context_and_context_equal_to_center(dev, dtype):
     tok = np.array(tok, dtype=np.int64)
     plan = _plan(tok, vocab, window, neg)
     assert any(ctx.count(ctx[0]) > 1 for ctx, _ in plan)
-    W_in, W_out = _tables(vocab, dim, 0.5, 3, dev)
+    W_in, W_out = tables(vocab, dim, 0.5, 3, dev)
     (rin, w_in, rout, w_out, loss), tol = _order_tolerance(W_in, W_out, dim, plan, lr, 4.0)
     a_, b_ = W_in.clone(), W_out.clone()
-    st, ts, nan = _fused(a_, b_, dim, torch.from_numpy(tok).to(dtype).to(dev), vocab, lr=lr, window=window, neg=neg)
+    st, ts, nan = fused(a_, b_, dim, torch.from_numpy(tok).to(dtype).to(dev), vocab, lr=lr, window=window, neg=neg,
+                        cbow=True)
     gi, go = a_[rin, :dim].cpu().numpy(), b_[rout, :dim].cpu().numpy()
     assert np.abs(gi - w_in).max() <= tol and np.abs(go - w_out).max() <= tol
     # the effect of a wrong update is far above the tolerance
@@ -345,11 +287,11 @@ def test_topic_corpus_call_matches_sequential_replay(dev):
     seq, pos, kept, dropped = R.compact(tok, vocab, p, 0, SEED, PH)
     plan = R.cbow_centers(seq, pos, window, neg, vocab, 0, SEED, PH, cdf=cdf.cpu().numpy(), last_nonzero=last)
     assert kept < (tok >= 0).sum()
-    W_in, W_out = _tables(vocab, dim, 0.5 / dim ** 0.5, 8, dev)
+    W_in, W_out = tables(vocab, dim, 0.5 / dim ** 0.5, 8, dev)
     (rin, w_in, rout, w_out, loss), tol = _order_tolerance(W_in, W_out, dim, plan, lr, 4.0)
     a, b = W_in.clone(), W_out.clone()
-    st, ts, nan = _fused(a, b, dim, torch.from_numpy(tok).to(dev), vocab, lr=lr, window=window, neg=neg, cdf=cdf,
-                         last=last, keep_p=torch.from_numpy(p).to(dev))
+    st, ts, nan = fused(a, b, dim, torch.from_numpy(tok).to(dev), vocab, lr=lr, window=window, neg=neg, cdf=cdf,
+                        last=last, keep_p=torch.from_numpy(p).to(dev), cbow=True)
     gi, go = a[rin, :dim].cpu().numpy(), b[rout, :dim].cpu().numpy()
     assert np.abs(gi - w_in).max() <= tol and np.abs(go - w_out).max() <= tol
     orig = R.cbow_update
@@ -385,16 +327,16 @@ def test_grid_stride_rounds_match_replay_and_default_grid(dev, dim):
     tok[:, :2] = np.random.default_rng(dim).permutation(vocab).reshape(n_sent, 2)
     tok = tok.reshape(-1)
     assert len(tok) > groups
-    W_in, W_out = _tables(vocab, dim, dim ** -0.25, 7, dev)
+    W_in, W_out = tables(vocab, dim, dim ** -0.25, 7, dev)
     w_in, w_out = W_in[:, :dim].double().cpu().numpy(), W_out[:, :dim].double().cpu().numpy()
     want = R.train_call(w_in, w_out, tok, lr=lr, window=5, negative_count=0, step=0, seed=SEED, philox=PH, cbow=True)
     tokens = torch.from_numpy(tok).to(dev)
     runs = []
     for reserve in (0, 1 << 20):
         a, b = W_in.clone(), W_out.clone()
-        st, ts, nan = _fused(a, b, dim, tokens, vocab, lr=lr, window=5, neg=0, reserve=reserve)
-        _close(a[:, :dim].cpu().numpy(), w_in, f"W_in, reserve {reserve}")
-        _close(b[:, :dim].cpu().numpy(), w_out, f"W_out, reserve {reserve}")
+        st, ts, nan = fused(a, b, dim, tokens, vocab, lr=lr, window=5, neg=0, reserve=reserve, cbow=True)
+        close(a[:, :dim].cpu().numpy(), w_in, f"W_in, reserve {reserve}")
+        close(b[:, :dim].cpu().numpy(), w_out, f"W_out, reserve {reserve}")
         assert st[1].item() == want["targets"] == 2 * n_sent
         assert abs(st[0].item() - want["loss"]) <= 1e-5 * want["loss"]
         assert ts.tolist() == [len(tok), 2 * n_sent, 2 * n_sent, 0] and nan == 0
@@ -411,16 +353,17 @@ def test_sentence_cut_by_both_ends_of_the_call(dev, dtype):
     1e-9, far inside the tolerance of 5e-7, while one context more or less moves rows by ~1e-6."""
     vocab, dim, neg, lr, window = 20000, 64, 3, 2e-4, 5
     tok = np.random.default_rng(3).permutation(vocab)[:9]
-    W_in, W_out = _tables(vocab, dim, 0.05, 5, dev)
+    W_in, W_out = tables(vocab, dim, 0.05, 5, dev)
     w_in, w_out = W_in[:, :dim].double().cpu().numpy(), W_out[:, :dim].double().cpu().numpy()
     want = R.train_call(w_in, w_out, tok, lr=lr, window=window, negative_count=neg, step=0, seed=SEED, philox=PH,
                         cbow=True)
     seq, pos, _, _ = R.compact(tok, vocab, None, 0, SEED, PH)
     r = R.radii(pos, window, 0, SEED, PH)
     assert sum(e - r[e] < 0 for e in range(9)) >= 2 and sum(e + r[e] > 8 for e in range(9)) >= 2
-    st, ts, nan = _fused(W_in, W_out, dim, torch.from_numpy(tok).to(dev, dtype), vocab, lr=lr, window=window, neg=neg)
-    _close(W_in[:vocab, :dim].cpu().numpy(), w_in, "W_in")
-    _close(W_out[:vocab, :dim].cpu().numpy(), w_out, "W_out")
+    st, ts, nan = fused(W_in, W_out, dim, torch.from_numpy(tok).to(dev, dtype), vocab, lr=lr, window=window, neg=neg,
+                        cbow=True)
+    close(W_in[:vocab, :dim].cpu().numpy(), w_in, "W_in")
+    close(W_out[:vocab, :dim].cpu().numpy(), w_out, "W_out")
     assert st[1].item() == want["targets"] and abs(st[0].item() - want["loss"]) <= 1e-5 * want["loss"]
     assert ts.tolist() == [9, 9, want["contexts"], 0] and nan == 0
 
@@ -440,10 +383,10 @@ def test_call_without_contexts_leaves_tables_and_stats_alone(dev, case, dtype):
         tok = np.array([3, -1, 4, 60, 5, -1, 6])
     else:
         tok = np.array([17])
-    W_in, W_out = _tables(vocab, dim, 0.5, 1, dev)
+    W_in, W_out = tables(vocab, dim, 0.5, 1, dev)
     in0, out0 = W_in.clone(), W_out.clone()
-    st, ts, nan = _fused(W_in, W_out, dim, torch.from_numpy(tok).to(dev, dtype), vocab, lr=0.1, window=5, neg=5,
-                         keep_p=torch.from_numpy(keep_p).to(dev) if keep_p is not None else None)
+    st, ts, nan = fused(W_in, W_out, dim, torch.from_numpy(tok).to(dev, dtype), vocab, lr=0.1, window=5, neg=5,
+                        keep_p=torch.from_numpy(keep_p).to(dev) if keep_p is not None else None, cbow=True)
     _, _, kept, dropped = R.compact(tok, vocab, keep_p, 0, SEED, PH)
     assert torch.equal(W_in, in0) and torch.equal(W_out, out0)
     assert st.tolist() == [0.0, 0.0] and nan == 0

@@ -1,7 +1,7 @@
-"""The fused skip-gram window kernel (``fps_w2v_window_kernel``) against the fp64 replay of ``models/w2v_ref.py``,
-every Philox draw replayed by ``tests/philox_ref.py``: every dispatch rung and the four ways a context's noise words
-are drawn and blocked, uniform and unigram noise, voided and repeated targets, grid-stride rounds, the ends of a
-call, and the counters."""
+"""The fused window kernel's skip-gram (``fps_w2v_kernel<false, ...>``) against the fp64 replay of
+``models/w2v_ref.py``, every Philox draw replayed by ``tests/philox_ref.py``: every dispatch rung and the four ways a
+context's noise words are drawn and blocked, uniform and unigram noise, voided and repeated targets, grid-stride
+rounds, the ends of a call, and the counters."""
 import functools
 
 import numpy as np
@@ -12,51 +12,15 @@ import fps_b200  # noqa: F401
 from fps_b200.models import w2v_ref as R
 from fps_b200.ops import native
 from tests.philox_ref import philox4x32 as PH
+from tests.w2v_cases import ATOL_OF_MAX, RTOL, RUNGS, SEED, SWEEP, VOCAB, close, fused, noise_dist, tables
 
 pytestmark = pytest.mark.gpu
-
-SEED = 4
-
-# fps_w2v_window_fused dispatches on the row stride (the dim rounded up to 4 floats; nvec = stride / 4 float4) to
-# fps_w2v_window_kernel<LPR, VPL, MINB, TB>: LPR lanes per row, VPL float4 per lane, MINB CTAs per SM and TB
-# target slots pulled per block.
-#   dim  stride  nvec  <LPR, VPL, MINB, TB>
-#     3      4     1   < 1, 1, 2, 8>   padding column 3
-#     4      4     1   < 1, 1, 2, 8>
-#     8      8     2   < 2, 1, 2, 8>
-#    13     16     4   < 4, 1, 2, 8>   padding columns 13-15
-#    16     16     4   < 4, 1, 2, 8>
-#    24     24     6   < 8, 1, 2, 8>   lanes 6-7 hold nothing
-#    36     36     9   <16, 1, 2, 8>   lanes 9-15 hold nothing
-#   100    100    25   <32, 1, 2, 8>   lanes 25-31 hold nothing
-#   136    136    34   <32, 2, 1, 8>   lanes 0-1 hold 2 float4, the others 1
-#   256    256    64   <32, 2, 1, 8>
-#   300    300    75   <32, 3, 1, 8>   lanes 0-10 hold 3 float4, the others 2
-#   387    388    97   <32, 4, 1, 6>   padding column 387; lane 0 holds 4 float4, the others 3
-#   388    388    97   <32, 4, 1, 6>
-#   512    512   128   <32, 4, 1, 6>
-RUNGS = {3: (1, 1, 8), 4: (1, 1, 8), 8: (2, 1, 8), 13: (4, 1, 8), 16: (4, 1, 8), 24: (8, 1, 8), 36: (16, 1, 8),
-         100: (32, 1, 8), 136: (32, 2, 8), 256: (32, 2, 8), 300: (32, 3, 8), 387: (32, 4, 6), 388: (32, 4, 6),
-         512: (32, 4, 6)}   # dim -> (LPR, VPL, TB)
-
 
 def _path(neg, lpr, tb):
     """How the kernel gets a context's noise words: lane j of the group draws word j and the others read it with a
     shuffle (negative <= LPR), or every lane draws all of them; the 1 + negative target slots fit one block of TB
     or take several."""
     return ("shuffled" if neg <= lpr else "serial", "one block" if 1 + neg <= tb else "several blocks")
-
-
-SWEEP = [(dim, neg) for dim, (lpr, _, _) in RUNGS.items() for neg in sorted({0, 1, lpr, lpr + 1, 7, 8, 20})]
-
-# The fp32 kernel against the fp64 replay: 2e-5 relative plus 1e-5 of the table's largest value.  The same replay
-# run in numpy fp32 stays within a tenth of this at dim 512 with 255 negatives, while a block one slot off or voids
-# compacted before blocking move rows by ~1e-3.
-RTOL, ATOL_OF_MAX = 2e-5, 1e-5
-
-
-def _close(got, want, what):
-    np.testing.assert_allclose(got, want, rtol=RTOL, atol=ATOL_OF_MAX * float(np.abs(want).max()), err_msg=what)
 
 
 @pytest.fixture
@@ -73,57 +37,14 @@ def test_sweep_reaches_every_rung_and_noise_path():
     assert {d for d in RUNGS if d % 4} == {3, 13, 387}
 
 
-def _tables(vocab, dim, scale, seed, dev):
-    """W_in and W_out ``[vocab, stride]`` fp32, uniform on +-scale, padding columns 0."""
-    g = torch.Generator(device=dev).manual_seed(seed)
-    out = []
-    for _ in range(2):
-        t = torch.zeros(vocab, (dim + 3) // 4 * 4, device=dev)
-        t[:, :dim] = (torch.rand(vocab, dim, generator=g, device=dev) * 2 - 1) * scale
-        out.append(t)
-    return out
-
-
-def _fused(W_in, W_out, dim, tokens, vocab, *, lr, window, neg, step=0, max_tries=32, cdf=None, last=0,
-           keep_p=None, reserve=0):
-    """One call through native.w2v_subsample + native.w2v_window_fused; returns (stats, token_stats, nan_flag)."""
-    dev = W_in.device
-    st = torch.zeros(2, dtype=torch.float32, device=dev)
-    ts = torch.zeros(4, dtype=torch.int64, device=dev)
-    nan = torch.zeros(1, dtype=torch.int32, device=dev)
-    seq, pos, n_comp = native.w2v_subsample(tokens, vocab, keep_p, seed=SEED, step=step, token_stats=ts)
-    native.w2v_window_fused(seq, pos, n_comp, native.local_table(W_in, dim), native.local_table(W_out, dim), lr,
-                            window=window, negative=neg, vocab=vocab, seed=SEED, step=step, cdf=cdf,
-                            last_nonzero=last, max_tries=max_tries, stats=st, token_stats=ts, nan_flag=nan,
-                            reserve_total=reserve)
-    torch.cuda.synchronize()
-    return st.cpu(), ts.cpu(), int(nan.item())
-
-
 # ---- every rung x every noise path, on corpora whose centers share no row --------------------------------------
-
-VOCAB = 100_000
-
-
-@functools.lru_cache(maxsize=None)
-def _noise(kind):
-    """(counts, cdf, last_nonzero) of the unigram noise: 30% of the words and the last 1000 have weight 0."""
-    if kind == "uniform":
-        return None, None, 0
-    g = np.random.default_rng(11)
-    c = g.integers(1, 50, size=VOCAB).astype(np.float64)
-    c[g.random(VOCAB) < 0.3] = 0.0
-    c[-1000:] = 0.0
-    cdf = native.noise_cdf(torch.from_numpy(c).cuda(), 0.75).cpu().numpy()
-    return c, cdf, int(np.flatnonzero(c)[-1])
-
 
 @functools.lru_cache(maxsize=None)
 def _corpus(neg, kind, n_sent=16):
     """Sentences ``x y -1`` whose centers read pairwise disjoint W_out rows, so no result depends on the order the
     lane-groups run in.  Built greedily at step 0: a candidate sentence that would read a row another center reads
     is replaced by a boundary.  Returns (tokens, [(center, its targets)])."""
-    _, cdf, last = _noise(kind)
+    _, cdf, last = noise_dist(kind)
     words = iter(np.random.default_rng(neg).permutation(VOCAB).tolist())
     tok, rep, used = [], [], set()
     while len(rep) < 2 * n_sent:
@@ -147,13 +68,13 @@ def test_window_kernel_matches_fp64_replay_at_every_rung(dev, dim, neg, noise):
     from fps_b200.models.w2v import DeviceSkipGram
 
     lr = 0.1
-    counts, cdf, last = _noise(noise)
+    counts, cdf, last = noise_dist(noise)
     tok, rep = _corpus(neg, noise)
     m = DeviceSkipGram(VOCAB, dim, learning_rate=lr, negative=neg, seed=SEED, noise_counts=counts, sample=0.0)
     try:
         if counts is not None:
             assert np.array_equal(m._noise_cdf.cpu().numpy(), cdf) and m._noise_last == last < VOCAB - 1
-        W_in, W_out = _tables(VOCAB, dim, dim ** -0.25, dim + neg, dev)
+        W_in, W_out = tables(VOCAB, dim, dim ** -0.25, dim + neg, dev)
         m.w_in.local.copy_(W_in)
         m.w_out.local.copy_(W_out)
         centers = [c for c, _ in rep]
@@ -170,8 +91,8 @@ def test_window_kernel_matches_fp64_replay_at_every_rung(dev, dim, neg, noise):
         m.train_tokens(torch.from_numpy(tok).to(dev), window=5)
         torch.cuda.synchronize()
         got_in, got_out = m.w_in.local, m.w_out.local
-        _close(got_in[centers, :dim].cpu().numpy(), w_in, "W_in")
-        _close(got_out[rows, :dim].cpu().numpy(), w_out, "W_out")
+        close(got_in[centers, :dim].cpu().numpy(), w_in, "W_in")
+        close(got_out[rows, :dim].cpu().numpy(), w_out, "W_out")
         keep_in = torch.ones(VOCAB, dtype=torch.bool, device=dev)
         keep_in[centers] = False
         keep_out = torch.ones(VOCAB, dtype=torch.bool, device=dev)
@@ -211,7 +132,7 @@ def test_void_and_repeated_targets_match_fp64_replay(dev, dim, neg, max_tries, n
     tokens = torch.tensor([x, y], device=dev)
     seen = set()
     for step in range(2 if neg == 255 else 6):
-        W_in, W_out = _tables(vocab, dim, 0.5, step, dev)
+        W_in, W_out = tables(vocab, dim, 0.5, step, dev)
         W_in[y] = 0.0
         in0 = W_in.cpu().numpy()
         w_in, w_out = W_in[:, :dim].double().cpu().numpy(), W_out[:, :dim].double().cpu().numpy()
@@ -219,11 +140,11 @@ def test_void_and_repeated_targets_match_fp64_replay(dev, dim, neg, max_tries, n
         noise_kw = dict(cdf=cdf, last_nonzero=last, max_tries=max_tries)
         want = R.train_call(w_in, w_out, [x, y], lr=lr, window=5, negative_count=neg, step=step, seed=SEED,
                             philox=PH, **noise_kw)
-        st, ts, nan = _fused(W_in, W_out, dim, tokens, vocab, lr=lr, window=5, neg=neg, step=step,
-                             max_tries=max_tries, cdf=cdf_d, last=last)
+        st, ts, nan = fused(W_in, W_out, dim, tokens, vocab, lr=lr, window=5, neg=neg, step=step,
+                            max_tries=max_tries, cdf=cdf_d, last=last)
         got_in, got_out = W_in.cpu().numpy(), W_out.cpu().numpy()
-        _close(got_out[:, :dim], w_out, f"W_out, step {step}")
-        _close(got_in[x, :dim], w_in[x], f"W_in[x], step {step}")
+        close(got_out[:, :dim], w_out, f"W_out, step {step}")
+        close(got_in[x, :dim], w_in[x], f"W_in[x], step {step}")
         sx = [t for t, _ in R.center_targets(0, [y], neg, vocab, step, SEED, PH, **noise_kw)[0]]
         sy = [t for t, _ in R.center_targets(1, [x], neg, vocab, step, SEED, PH, **noise_kw)[0]]
         bound = 0.5 * lr * lr * np.abs(u_x) * sum(sx.count(t) for t in sy if t >= 0)
@@ -261,16 +182,16 @@ def test_grid_stride_rounds_match_replay_and_default_grid(dev, dim):
     tok[:, :2] = np.random.default_rng(dim).permutation(vocab).reshape(n_sent, 2)
     tok = tok.reshape(-1)
     assert len(tok) > groups
-    W_in, W_out = _tables(vocab, dim, dim ** -0.25, 7, dev)
+    W_in, W_out = tables(vocab, dim, dim ** -0.25, 7, dev)
     w_in, w_out = W_in[:, :dim].double().cpu().numpy(), W_out[:, :dim].double().cpu().numpy()
     want = R.train_call(w_in, w_out, tok, lr=lr, window=5, negative_count=0, step=0, seed=SEED, philox=PH)
     tokens = torch.from_numpy(tok).to(dev)
     runs = []
     for reserve in (0, 1 << 20):
         a, b = W_in.clone(), W_out.clone()
-        st, ts, nan = _fused(a, b, dim, tokens, vocab, lr=lr, window=5, neg=0, reserve=reserve)
-        _close(a[:, :dim].cpu().numpy(), w_in, f"W_in, reserve {reserve}")
-        _close(b[:, :dim].cpu().numpy(), w_out, f"W_out, reserve {reserve}")
+        st, ts, nan = fused(a, b, dim, tokens, vocab, lr=lr, window=5, neg=0, reserve=reserve)
+        close(a[:, :dim].cpu().numpy(), w_in, f"W_in, reserve {reserve}")
+        close(b[:, :dim].cpu().numpy(), w_out, f"W_out, reserve {reserve}")
         assert st[1].item() == want["targets"] == 2 * n_sent
         assert abs(st[0].item() - want["loss"]) <= 1e-5 * want["loss"]
         assert ts.tolist() == [len(tok), 2 * n_sent, 2 * n_sent, 0] and nan == 0
@@ -293,7 +214,7 @@ def test_sentence_cut_by_both_ends_of_the_call(dev, dtype):
     tok = np.random.default_rng(3).permutation(vocab)[:9]
     m = DeviceSkipGram(vocab, dim, learning_rate=lr, negative=neg, seed=SEED, sample=0.0)
     try:
-        W_in, W_out = _tables(vocab, dim, 0.05, 5, dev)
+        W_in, W_out = tables(vocab, dim, 0.05, 5, dev)
         m.w_in.local.copy_(W_in)
         m.w_out.local.copy_(W_out)
         w_in, w_out = W_in[:, :dim].double().cpu().numpy(), W_out[:, :dim].double().cpu().numpy()
@@ -305,8 +226,8 @@ def test_sentence_cut_by_both_ends_of_the_call(dev, dtype):
         assert sum(e - r[e] < 0 for e, _ in wins) >= 2 and sum(e + r[e] > 8 for e, _ in wins) >= 2
         m.train_tokens(torch.from_numpy(tok).to(dev, dtype), window=window)
         torch.cuda.synchronize()
-        _close(m.w_in.local[:vocab, :dim].cpu().numpy(), w_in, "W_in")
-        _close(m.w_out.local[:vocab, :dim].cpu().numpy(), w_out, "W_out")
+        close(m.w_in.local[:vocab, :dim].cpu().numpy(), w_in, "W_in")
+        close(m.w_out.local[:vocab, :dim].cpu().numpy(), w_out, "W_out")
         st = m.stats.cpu()
         assert st[1].item() == want["targets"] == want["contexts"] * (1 + neg)
         assert abs(st[0].item() - want["loss"]) <= 1e-5 * want["loss"]
@@ -328,10 +249,10 @@ def test_call_without_contexts_leaves_tables_and_stats_alone(dev, case, dtype):
         keep_p = np.zeros(vocab)
     else:
         tok = np.array([17])
-    W_in, W_out = _tables(vocab, dim, 0.5, 1, dev)
+    W_in, W_out = tables(vocab, dim, 0.5, 1, dev)
     in0, out0 = W_in.clone(), W_out.clone()
-    st, ts, nan = _fused(W_in, W_out, dim, torch.from_numpy(tok).to(dev, dtype), vocab, lr=0.1, window=5, neg=5,
-                         keep_p=torch.from_numpy(keep_p).to(dev) if keep_p is not None else None)
+    st, ts, nan = fused(W_in, W_out, dim, torch.from_numpy(tok).to(dev, dtype), vocab, lr=0.1, window=5, neg=5,
+                        keep_p=torch.from_numpy(keep_p).to(dev) if keep_p is not None else None)
     _, _, kept, dropped = R.compact(tok, vocab, keep_p, 0, SEED, PH)
     assert torch.equal(W_in, in0) and torch.equal(W_out, out0)
     assert st.tolist() == [0.0, 0.0] and nan == 0

@@ -85,13 +85,14 @@ def _layout(tmp_path, header, lines):
 
 
 STRUCT_HEADER = {"MfArgs": "fps_mf_args.cuh", "BprArgs": "fps_mf_args.cuh", "ExchArgs": "fps_replica.cu",
-                 "FlushPolicy": "fps_replica.cu", "BucketArgs": "fps_bucket.cu"}   # where each struct lives
+                 "FlushPolicy": "fps_replica.cu", "BucketArgs": "fps_bucket.cu",
+                 "W2vArgs": "fps_w2v_window.cu"}   # where each struct lives
 
 
 @pytest.mark.skipif(_nvcc() is None, reason="nvcc not found")
 @pytest.mark.parametrize("struct, mirror", [
     ("MfArgs", native.MfArgsC), ("BprArgs", native.BprArgsC), ("ExchArgs", native.ExchArgsC),
-    ("FlushPolicy", native.FlushPolicyC), ("BucketArgs", native.BucketArgsC)])
+    ("FlushPolicy", native.FlushPolicyC), ("BucketArgs", native.BucketArgsC), ("W2vArgs", native.W2vArgsC)])
 def test_args_mirror_matches_the_c_layout(tmp_path, struct, mirror):
     lines = [f'  printf("sizeof %zu\\n", sizeof({struct}));']
     lines += [f'  printf("{f} %zu\\n", offsetof({struct}, {f}));' for f, _ in mirror._fields_]
